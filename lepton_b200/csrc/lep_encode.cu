@@ -392,6 +392,9 @@ lep_encode_kernel(const ImageDesc* __restrict__ images, SegDesc* __restrict__ se
                     const int adv = adv_unpredict(dc_h, false, dp.pred);
                     if (act_h && dc_h != adv_unpredict((int)(int16_t)adv, true, dp.pred)) status = ST_COEF_RANGE;
                     dc_v = (int)(int16_t)adv;
+                    // a residual that round-trips can still need more than 11 bits (adv_unpredict wraps only once, and a
+                    // large prediction leaves it far outside +-1024): the reference refuses it too (encoder.cc:341-343)
+                    if (act_h && bitlen(iabs(dc_v) & 0xffff) > 11) status = ST_COEF_RANGE;
                     dc_len = min(bitlen(iabs(dc_v) & 0xffff), 11);
                 }
                 const int n_dc = coef_entries(dc_len);

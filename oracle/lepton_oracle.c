@@ -246,11 +246,85 @@ static inline int code_bit(Codec *c, Branch *b, int bit) {
     return bit;
 }
 
+/* ------------------------------------------------------------------ regime counters
+ * Each site below is a place where the reference's arithmetic wraps, truncates or caps.  Beside the wrapped value the
+ * oracle computes the exact one (int64, no cap); when they differ the site's counter goes up.  The counters change
+ * nothing that is coded: they show which of these regimes a test input really reaches.  (The cap of 16 on the bit length
+ * of the DC offset uncertainty has no site: the estimates are int16, so |unc2| <= 32768 and its bit length never
+ * exceeds 16.) */
+enum {
+    RG_IDCT_INT32_WRAP,      /* an IDCT output whose int32 computation wrapped */
+    RG_IDCT_INT16_PIXEL,     /* an IDCT output pixel that does not fit the int16 it is stored in */
+    RG_DC_EST_INT16,         /* a DC estimate from a neighbour edge pixel that wrapped in int16 */
+    RG_EDGE_INT16,           /* an edge pixel of the neighbour summary that wrapped in int16 */
+    RG_QDC_INT16,            /* q0 * dc wrapped in int16 */
+    RG_LAK_UINT32_WRAP,      /* the Lakhani predictor's sum wrapped in 32 bits */
+    RG_SIGN_CTX_INT16,       /* (int16_t)prior of the edge sign context differs from prior */
+    RG_THR_CTX_MASK,         /* |prior| > 0xffff: the threshold context keeps only its low 16 bits */
+    RG_THR_CTX_CAP255,       /* the threshold context (|prior| & 0xffff) >> min_thr capped at 255 */
+    RG_BSR_CAP1023,          /* |prior| capped at 1023 for the exponent context */
+    RG_LEN_MXM_CAP11,        /* DC uncertainty bit length capped at 11 */
+    RG_THR_SO_SAT127,        /* the threshold bits' context index saturated at 127 */
+    RG_ADV_WRAP_POS,         /* adv_unpredict wrapped a value above +1024 */
+    RG_ADV_WRAP_NEG,         /* adv_unpredict wrapped a value below -1024 */
+    RG_AC_LEN11,             /* an AC coefficient of the largest codable length, 11 */
+    RG_REFUSE_DC,            /* status 6: a DC that adv_unpredict cannot round-trip */
+    RG_REFUSE_DC_LEN,        /* status 6: a DC residual that round-trips but is longer than 11 bits */
+    RG_REFUSE_AC,            /* status 6: a coefficient longer than 11 bits */
+    RG_COUNT
+};
+static const char *const k_regime_names[RG_COUNT] = {
+    "idct_int32_wrap", "idct_int16_pixel", "dc_est_int16", "edge_int16", "qdc_int16", "lak_uint32_wrap",
+    "sign_ctx_int16", "thr_ctx_mask", "thr_ctx_cap255", "bsr_cap1023", "len_mxm_cap11",
+    "thr_so_sat127", "adv_wrap_pos", "adv_wrap_neg", "ac_len11", "refuse_dc", "refuse_dc_len", "refuse_ac"};
+static uint64_t g_regime[RG_COUNT];
+#define REGIME(site, cond) do { if (cond) ++g_regime[site]; } while (0)
+
 /* ------------------------------------------------------------------ IDCT (src/lepton/idct.cc:36-161; SSE form :196-355) */
+/* the same IDCT in exact int64 arithmetic (nothing wraps): what idct_sans_dc would give without its int32 wrap */
+static void idct_exact(const int16_t *blk /*aligned*/, const uint16_t q[64], int64_t out[64]) {
+    const int64_t w1 = 2841, w2 = 2676, w3 = 2408, w5 = 1609, w6 = 1108, w7 = 565, r2 = 181;
+    int64_t im[64];
+    for (int y = 0; y < 8; ++y) {
+        int64_t c[8];
+        for (int i = 0; i < 8; ++i) c[i] = (y == 0 && i == 0) ? 0 : (int64_t)blk[k_raster_to_aligned[y * 8 + i]] * q[y * 8 + i];
+        int64_t x0 = c[0] * 2048 + 128, x1 = c[4] * 2048, x2 = c[6], x3 = c[2], x4 = c[1], x5 = c[7], x6 = c[5], x7 = c[3];
+        int64_t x8 = w7 * (x4 + x5);
+        x4 = x8 + (w1 - w7) * x4; x5 = x8 - (w1 + w7) * x5;
+        x8 = w3 * (x6 + x7);
+        x6 = x8 - (w3 - w5) * x6; x7 = x8 - (w3 + w5) * x7;
+        x8 = x0 + x1; x0 -= x1;
+        x1 = w6 * (x3 + x2);
+        x2 = x1 - (w2 + w6) * x2; x3 = x1 + (w2 - w6) * x3;
+        x1 = x4 + x6; x4 -= x6; x6 = x5 + x7; x5 -= x7;
+        x7 = x8 + x3; x8 -= x3; x3 = x0 + x2; x0 -= x2;
+        x2 = (r2 * (x4 + x5) + 128) >> 8; x4 = (r2 * (x4 - x5) + 128) >> 8;
+        int64_t *o = im + y * 8;
+        o[0] = (x7 + x1) >> 8; o[1] = (x3 + x2) >> 8; o[2] = (x0 + x4) >> 8; o[3] = (x8 + x6) >> 8;
+        o[4] = (x8 - x6) >> 8; o[5] = (x0 - x4) >> 8; o[6] = (x3 - x2) >> 8; o[7] = (x7 - x1) >> 8;
+    }
+    for (int x = 0; x < 8; ++x) {
+        int64_t y0 = im[x] * 256 + 8192, y1 = im[32 + x] * 256;
+        int64_t y2 = im[48 + x], y3 = im[16 + x], y4 = im[8 + x], y5 = im[56 + x], y6 = im[40 + x], y7 = im[24 + x];
+        int64_t y8 = w7 * (y4 + y5) + 4;
+        y4 = (y8 + (w1 - w7) * y4) >> 3; y5 = (y8 - (w1 + w7) * y5) >> 3;
+        y8 = w3 * (y6 + y7) + 4;
+        y6 = (y8 - (w3 - w5) * y6) >> 3; y7 = (y8 - (w3 + w5) * y7) >> 3;
+        y8 = y0 + y1; y0 -= y1;
+        y1 = w6 * (y3 + y2) + 4;
+        y2 = (y1 - (w2 + w6) * y2) >> 3; y3 = (y1 + (w2 - w6) * y3) >> 3;
+        y1 = y4 + y6; y4 -= y6; y6 = y5 + y7; y5 -= y7;
+        y7 = y8 + y3; y8 -= y3; y3 = y0 + y2; y0 -= y2;
+        y2 = (r2 * (y4 + y5) + 128) >> 8; y4 = (r2 * (y4 - y5) + 128) >> 8;
+        out[x] = (y7 + y1) >> 11; out[8 + x] = (y3 + y2) >> 11; out[16 + x] = (y0 + y4) >> 11; out[24 + x] = (y8 + y6) >> 11;
+        out[32 + x] = (y8 - y6) >> 11; out[40 + x] = (y0 - y4) >> 11; out[48 + x] = (y3 - y2) >> 11; out[56 + x] = (y7 - y1) >> 11;
+    }
+}
+
 static void idct_sans_dc(const int16_t *blk /*aligned*/, const uint16_t q[64], int16_t outp[64]) {
     enum { w1 = 2841, w2 = 2676, w3 = 2408, w5 = 1609, w6 = 1108, w7 = 565, r2 = 181,
            w1pw7 = w1 + w7, w1mw7 = w1 - w7, w2pw6 = w2 + w6, w2mw6 = w2 - w6, w3pw5 = w3 + w5, w3mw5 = w3 - w5 };
-    int32_t im[64];
+    int32_t im[64], wide[64];
 #define CR(i) ((int32_t)blk[k_raster_to_aligned[i]])
 #define U(x) ((uint32_t)(x))
     for (int y = 0; y < 8; ++y) {
@@ -318,14 +392,21 @@ static void idct_sans_dc(const int16_t *blk /*aligned*/, const uint16_t q[64], i
         y0 = (int32_t)(U(y0) - U(y2));
         y2 = (int32_t)(U(r2) * U(y4 + y5) + 128u) >> 8;
         y4 = (int32_t)(U(r2) * U(y4 - y5) + 128u) >> 8;
-        outp[x] = (int16_t)((int32_t)(U(y7) + U(y1)) >> 11);
-        outp[8 + x] = (int16_t)((int32_t)(U(y3) + U(y2)) >> 11);
-        outp[16 + x] = (int16_t)((int32_t)(U(y0) + U(y4)) >> 11);
-        outp[24 + x] = (int16_t)((int32_t)(U(y8) + U(y6)) >> 11);
-        outp[32 + x] = (int16_t)((int32_t)(U(y8) - U(y6)) >> 11);
-        outp[40 + x] = (int16_t)((int32_t)(U(y0) - U(y4)) >> 11);
-        outp[48 + x] = (int16_t)((int32_t)(U(y3) - U(y2)) >> 11);
-        outp[56 + x] = (int16_t)((int32_t)(U(y7) - U(y1)) >> 11);
+        wide[x] = ((int32_t)(U(y7) + U(y1)) >> 11);
+        wide[8 + x] = ((int32_t)(U(y3) + U(y2)) >> 11);
+        wide[16 + x] = ((int32_t)(U(y0) + U(y4)) >> 11);
+        wide[24 + x] = ((int32_t)(U(y8) + U(y6)) >> 11);
+        wide[32 + x] = ((int32_t)(U(y8) - U(y6)) >> 11);
+        wide[40 + x] = ((int32_t)(U(y0) - U(y4)) >> 11);
+        wide[48 + x] = ((int32_t)(U(y3) - U(y2)) >> 11);
+        wide[56 + x] = ((int32_t)(U(y7) - U(y1)) >> 11);
+    }
+    int64_t exact[64];
+    idct_exact(blk, q, exact);
+    for (int i = 0; i < 64; ++i) {
+        outp[i] = (int16_t)wide[i];
+        REGIME(RG_IDCT_INT32_WRAP, wide[i] != exact[i]);
+        REGIME(RG_IDCT_INT16_PIXEL, outp[i] != wide[i]);
     }
 #undef CR
 #undef U
@@ -372,10 +453,13 @@ static int32_t lak(const BlockCtx *b, const QuantTables *qt, int band) {
         return 0;
     }
     uint32_t pred = (uint32_t)ca[0] * (uint32_t)icos[0];
+    int64_t exact = (int64_t)ca[0] * icos[0];
     for (int i = 1; i < 8; ++i) {
         int sign = (i & 1) ? 1 : -1;
         pred -= (uint32_t)icos[i] * (uint32_t)(cx[i] + sign * ca[i]);
+        exact -= (int64_t)icos[i] * (cx[i] + sign * ca[i]);
     }
+    REGIME(RG_LAK_UINT32_WRAP, (int32_t)pred != exact);
     return (int32_t)pred / icos[0];
 }
 
@@ -397,6 +481,7 @@ static int adv_predict_dc_pix(const BlockCtx *b, const QuantTables *qt, int16_t 
                 int16_t delta = (int16_t)(pix[i] - pix[i + 8]);
                 int16_t recentered = (int16_t)(pix[i] + 1024);
                 dst[i] = (int16_t)((int16_t)(b->ns_above->edge[8 + i] - half_rz16(delta)) - recentered);
+                REGIME(RG_DC_EST_INT16, dst[i] != b->ns_above->edge[8 + i] - (pix[i] - pix[i + 8]) / 2 - (pix[i] + 1024));
             }
         }
         if (has_left) {
@@ -404,6 +489,7 @@ static int adv_predict_dc_pix(const BlockCtx *b, const QuantTables *qt, int16_t 
                 int16_t delta = (int16_t)(pix[i * 8] - pix[i * 8 + 1]);
                 int16_t recentered = (int16_t)(pix[i * 8] + 1024);
                 est[i] = (int16_t)((int16_t)(b->ns_left->edge[i] - half_rz16(delta)) - recentered);
+                REGIME(RG_DC_EST_INT16, est[i] != b->ns_left->edge[i] - (pix[i * 8] - pix[i * 8 + 1]) / 2 - (pix[i * 8] + 1024));
             }
         }
         int32_t avg_h_v[2] = {0, 0};
@@ -434,6 +520,8 @@ static int adv_predict_dc_pix(const BlockCtx *b, const QuantTables *qt, int16_t 
 static inline int adv_unpredict(int16_t saved_dc, int recover, int pred) {
     int max_value = 1 << 10, min_value = -max_value, adj = 2 * max_value + 1;
     int r = saved_dc + (recover ? pred : -pred);
+    REGIME(RG_ADV_WRAP_NEG, r < min_value);
+    REGIME(RG_ADV_WRAP_POS, r > max_value);
     if (r < min_value) r += adj;
     if (r > max_value) r -= adj;
     return r;
@@ -442,11 +530,15 @@ static inline int adv_unpredict(int16_t saved_dc, int recover, int pred) {
 /* NeighborSummary::set_horizontal / set_vertical, block_context.hh:44-78 (SSE: 16-bit lanes) */
 static void ns_set_edges(NeighborSummary *ns, const int16_t pix[64], const uint16_t q[64], int16_t dc) {
     int16_t qdc = (int16_t)((uint16_t)q[0] * (uint16_t)dc);
+    const int64_t qdc_exact = (int64_t)q[0] * dc;
+    REGIME(RG_QDC_INT16, qdc != qdc_exact);
     for (int i = 0; i < 8; ++i) {
         int16_t delta = (int16_t)(pix[56 + i] - pix[48 + i]);
         ns->edge[8 + i] = (int16_t)(pix[56 + i] + half_rz16(delta) + 1024 + qdc);
+        REGIME(RG_EDGE_INT16, ns->edge[8 + i] != pix[56 + i] + (pix[56 + i] - pix[48 + i]) / 2 + 1024 + qdc_exact);
         int16_t deltav = (int16_t)(pix[i * 8 + 7] - pix[i * 8 + 6]);
         ns->edge[i] = (int16_t)(pix[i * 8 + 7] + half_rz16(deltav) + 1024 + qdc);
+        REGIME(RG_EDGE_INT16, ns->edge[i] != pix[i * 8 + 7] + (pix[i * 8 + 7] - pix[i * 8 + 6]) / 2 + 1024 + qdc_exact);
     }
 }
 
@@ -487,6 +579,7 @@ static void code_one_edge(Codec *c, int cmp, int ci, const BlockCtx *b, int16_t 
         int32_t prior = lak(b, qt, coord);
         int nzbin = ne;
         int bsr = bit_length((uint32_t)imin(iabs(prior), 1023));
+        REGIME(RG_BSR_CAP1023, iabs(prior) > 1023);
         Branch *exp = c->model->exp_x[ci][nzbin][zig15][bsr];
         int16_t coef = c->encode ? b->here[aligned_off + lane] : 0;
         uint16_t abs_coef = (uint16_t)iabs(coef);
@@ -499,6 +592,8 @@ static void code_one_edge(Codec *c, int cmp, int ci, const BlockCtx *b, int16_t 
             dec_len = i + 1;
         }
         if (c->encode) {
+            REGIME(RG_AC_LEN11, length == 11);
+            REGIME(RG_REFUSE_AC, length > 11);
             if (length > 11) { c->err = LO_COEFFICIENT_OUT_OF_RANGE; return; }
             nonzero = coef != 0;
         } else {
@@ -507,6 +602,7 @@ static void code_one_edge(Codec *c, int cmp, int ci, const BlockCtx *b, int16_t 
         if (nonzero) {
             int min_thr = qt->min_noise_threshold[coord];
             int16_t v16 = (int16_t)prior; /* sign_array_8, model.hh:1114-1122: int16 truncation of best_prior */
+            REGIME(RG_SIGN_CTX_INT16, v16 != prior);
             int sctx = v16 == 0 ? 0 : (v16 > 0 ? 1 : 2);
             int sbit = code_bit(c, &c->model->sign[ci][sctx][bsr], coef >= 0);
             int neg = !sbit;
@@ -516,12 +612,15 @@ static void code_one_edge(Codec *c, int cmp, int ci, const BlockCtx *b, int16_t 
                 int i = length - 2;
                 if (i >= min_thr) {
                     uint16_t ctx_abs = (uint16_t)iabs(prior); /* residual_thresh_array, model.hh:1072-1088 */
+                    REGIME(RG_THR_CTX_MASK, ctx_abs != (int64_t)iabs(prior));
+                    REGIME(RG_THR_CTX_CAP255, (ctx_abs >> min_thr) > 255);
                     Branch *thr = c->model->res_thresh[ci][imin(ctx_abs >> min_thr, 255)][imin(length - min_thr, 7)];
                     unsigned so = 1;
                     for (; i >= min_thr; --i) {
                         int bit = code_bit(c, &thr[so], (abs_coef >> i) & 1);
                         val |= bit << i;
                         so = (so << 1) | (unsigned)bit;
+                        REGIME(RG_THR_SO_SAT127, so > 127);
                         if (so > 127) so = 127;
                     }
                 }
@@ -563,6 +662,7 @@ static void code_block(Codec *c, int cmp, const BlockCtx *b, int16_t *here_mut) 
         int16_t prior = aavrg(b, zz);
         int nzbin = k_nonzero_to_bin[left_nz];
         int bsr = bit_length((uint32_t)imin(iabs(prior), 1023));
+        REGIME(RG_BSR_CAP1023, iabs(prior) > 1023);
         Branch *exp = c->model->exp7x7[ci][nzbin][zz][bsr];
         int16_t coef = c->encode ? b->here[zz] : 0;
         uint16_t abs_coef = (uint16_t)iabs(coef);
@@ -574,6 +674,8 @@ static void code_block(Codec *c, int cmp, const BlockCtx *b, int16_t *here_mut) 
             dec_len = i + 1;
         }
         if (c->encode) {
+            REGIME(RG_AC_LEN11, length == 11);
+            REGIME(RG_REFUSE_AC, length > 11);
             if (length > 11) { c->err = LO_COEFFICIENT_OUT_OF_RANGE; return; }
             nonzero = length != 0;
         } else {
@@ -608,7 +710,7 @@ static void code_block(Codec *c, int cmp, const BlockCtx *b, int16_t *here_mut) 
     int16_t coef = 0;
     if (c->encode) {
         int adv = adv_unpredict(b->here[49], 0, pred);
-        if (b->here[49] != adv_unpredict((int16_t)adv, 1, pred)) { c->err = LO_COEFFICIENT_OUT_OF_RANGE; return; }
+        if (b->here[49] != adv_unpredict((int16_t)adv, 1, pred)) { ++g_regime[RG_REFUSE_DC]; c->err = LO_COEFFICIENT_OUT_OF_RANGE; return; }
         coef = (int16_t)adv;
     }
     {
@@ -616,6 +718,7 @@ static void code_block(Codec *c, int cmp, const BlockCtx *b, int16_t *here_mut) 
         int length = bit_length(abs_coef), dec_len = 0, nonzero = 0;
         int len_mxm = bit_length((uint16_t)iabs(unc));   /* uint16bit_length(abs(uncertainty)), encoder.cc:322 */
         int len_off = bit_length((uint16_t)iabs(unc2));
+        REGIME(RG_LEN_MXM_CAP11, len_mxm > 11);
         Branch *exp = c->model->exp_dc[imin(len_mxm, 11)][imin(len_off, 16)]; /* model.hh:520-529 */
         for (int i = 0; i < 11; ++i) {
             int bit = code_bit(c, &exp[i], length != i);
@@ -624,6 +727,7 @@ static void code_block(Codec *c, int cmp, const BlockCtx *b, int16_t *here_mut) 
             dec_len = i + 1;
         }
         if (c->encode) {
+            REGIME(RG_REFUSE_DC_LEN, length > 11);
             if (length > 11) { c->err = LO_COEFFICIENT_OUT_OF_RANGE; return; }
             nonzero = length != 0;
         } else {
@@ -799,3 +903,9 @@ int lo_decode_segment(const lo_geometry *g, int16_t *const planes[3], int min_y,
 }
 
 size_t lo_model_bytes(void) { return sizeof(Model); }
+
+/* regime counters: names, values (since the last reset), reset */
+int lo_regime_count(void) { return RG_COUNT; }
+const char *lo_regime_name(int i) { return i >= 0 && i < RG_COUNT ? k_regime_names[i] : NULL; }
+uint64_t lo_regime_value(int i) { return i >= 0 && i < RG_COUNT ? g_regime[i] : 0; }
+void lo_regime_reset(void) { memset(g_regime, 0, sizeof(g_regime)); }

@@ -92,3 +92,16 @@ def decode_segment(g: Geometry, planes, min_y, max_y, is_last, stream: bytes):
     rc = lib().lo_decode_segment(ctypes.byref(g), _ptrs(planes), min_y, max_y, int(is_last),
                                  buf.ctypes.data if len(buf) else None, len(buf), ctypes.byref(nd))
     return rc, nd.value
+
+
+def regime_counts(reset=False):
+    """{site: count} since the last reset: how often each place where the reference's arithmetic wraps, truncates or
+    caps (int32 IDCT, int16 pixels and edges, uint32 Lakhani sum, context masks and caps, DC wrap, status 6) produced a
+    value different from the exact one, over every segment the oracle coded.  reset=True clears them afterwards."""
+    L = lib()
+    L.lo_regime_name.restype = ctypes.c_char_p
+    L.lo_regime_value.restype = ctypes.c_uint64
+    out = {L.lo_regime_name(i).decode(): int(L.lo_regime_value(i)) for i in range(L.lo_regime_count())}
+    if reset:
+        L.lo_regime_reset()
+    return out

@@ -11,6 +11,8 @@ import oracle
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 GOLDEN = os.path.join(ROOT, "tests", "golden")
 MANIFEST = json.load(open(os.path.join(GOLDEN, "manifest.json")))
+# baseline JPEGs at the coder's numeric limits and what the reference CLI made of them (tests/golden/make_extremes.py)
+EXTREMES = json.load(open(os.path.join(GOLDEN, "extremes.json")))
 
 
 def golden_leps():
@@ -20,6 +22,28 @@ def golden_leps():
 
 def load_lep(name):
     return lepfmt.parse_container(open(os.path.join(GOLDEN, name), "rb").read())
+
+
+def read_golden(rel):
+    with open(os.path.join(GOLDEN, rel), "rb") as f:
+        return f.read()
+
+
+def extreme_jpegs():
+    """Names of the extreme JPEGs, refused ones included."""
+    return sorted(n for n in EXTREMES if n.endswith(".jpg"))
+
+
+def extreme_leps():
+    """(name of the .lep, name of its source JPEG) for every reference-written .lep of the extreme corpus: one per
+    accepted JPEG plus the multi-segment records."""
+    out = [(n[:-4] + ".lep", n) for n in extreme_jpegs() if EXTREMES[n]["status_want"] == 0]
+    out += [(n, e["source"]) for n, e in EXTREMES.items() if n.endswith(".lep")]
+    return sorted(out)
+
+
+def load_extreme_lep(name):
+    return lepfmt.parse_container(read_golden("extremes/" + name))
 
 
 def geometry_of(lf):
@@ -63,24 +87,40 @@ def coef_image_from_lep(lf, planes):
 
 
 def random_coef_image(rng, ncmp=3, mcuh=5, mcuv=4, sf=((2, 2), (1, 1), (1, 1)), density=0.25, amp=60, nseg=1,
-                      qscale=1):
-    """Synthetic coefficient planes with JPEG-like statistics (sparse, decaying with frequency)."""
+                      qscale=1, q16=False, max_cat=0, dc_max=1000):
+    """Synthetic coefficient planes with JPEG-like statistics (sparse, decaying with frequency).
+
+    The knobs that leave photo statistics behind: q16 draws every quantiser uniformly from the 16-bit range 1..65535;
+    max_cat > 0 draws the magnitude category of every kept coefficient uniformly from 0..max_cat (then uniformly inside the
+    category) instead of the geometric magnitudes; dc_max bounds the DC random walk (up to 2047; values beyond 1024 make
+    the reference refuse the segment with status 6)."""
     from lepton_b200 import CoefImage
     bch = [mcuh * sf[c][0] for c in range(ncmp)]
     bcv = [mcuv * sf[c][1] for c in range(ncmp)]
     planes = []
     for c in range(ncmp):
         n = bch[c] * bcv[c]
-        mag = rng.geometric(0.15, size=(n, 64)).astype(np.int32) * amp // 8
+        if max_cat:
+            cat = rng.integers(0, max_cat + 1, size=(n, 64))
+            lo = np.where(cat > 0, 1 << np.maximum(cat - 1, 0), 0)
+            mag = (lo + rng.integers(0, 1 << 16, size=(n, 64)) % np.maximum(lo, 1) * (cat > 0)).astype(np.int32)
+        else:
+            mag = rng.geometric(0.15, size=(n, 64)).astype(np.int32) * amp // 8
         decay = np.ones(64)
         decay[:49] = np.linspace(1.0, 0.05, 49)       # aligned order == zig-zag order for the 7x7 part
         keep = rng.random((n, 64)) < (density * decay + 0.02)
         sign = rng.integers(0, 2, size=(n, 64)) * 2 - 1
         p = (mag * keep * sign).astype(np.int16)
-        p[:, 49] = np.clip(np.cumsum(rng.integers(-20, 21, size=n)), -1000, 1000).astype(np.int16)  # smooth DC
         p = np.clip(p, -2047, 2047).astype(np.int16)
+        if dc_max > 1000:
+            p[:, 49] = rng.integers(-dc_max, dc_max + 1, size=n)
+        else:
+            p[:, 49] = np.clip(np.cumsum(rng.integers(-20, 21, size=n)), -dc_max, dc_max)  # smooth DC
         planes.append(np.ascontiguousarray(p))
-    q = [[max(1, min(255, int((3 + i // 4) * qscale))) for i in range(64)] for _ in range(ncmp)]
+    if q16:
+        q = [[int(v) for v in rng.integers(1, 65536, size=64)] for _ in range(ncmp)]
+    else:
+        q = [[max(1, min(255, int((3 + i // 4) * qscale))) for i in range(64)] for _ in range(ncmp)]
     v0 = bcv[0] // mcuv
     starts = sorted({(k * mcuv // nseg) * v0 for k in range(nseg)})
     return CoefImage(ncmp=ncmp, mcuv=mcuv, bch=bch, bcv=bcv, qtables_zigzag=q, planes=planes, luma_y_start=starts)

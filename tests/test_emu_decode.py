@@ -15,8 +15,8 @@ import pytest
 sys.path.insert(0, os.path.join(os.path.dirname(os.path.abspath(__file__)), "emu"))
 import emu  # noqa: E402
 import oracle  # noqa: E402
-from helpers import (coef_image_from_lep, geometry_of, golden_leps, load_lep, oracle_decode_planes, oracle_encode_image,
-                     random_coef_image, segments_of)
+from helpers import (EXTREMES, coef_image_from_lep, extreme_leps, geometry_of, golden_leps, load_extreme_lep, load_lep,
+                     oracle_decode_planes, oracle_encode_image, plane_hashes, random_coef_image, segments_of)
 
 KERNELS = [emu.KERNEL_WARP]
 GROUPS = [emu.KERNEL_G2(g) for g in (1, 2, 4, 8, 16, 32)]       # lep_decode_g2_kernel<G>; the library ships G = 4, 8, 32
@@ -116,3 +116,45 @@ def test_damaged_streams_end_the_same_way_in_all_kernels_and_the_oracle():
             for c in range(len(planes)):
                 assert np.array_equal(a[2][c], want[c])
     assert seen_bad > 0       # the damage was enough to hit the inconsistent-stream exit at least once
+
+
+@pytest.mark.parametrize("kernel", KERNELS + GROUPS)
+def test_extreme_corpus_decodes_to_the_reference_planes(kernel):
+    """Every reference-written .lep of the extreme corpus (1, 4 and 8 thread-segments) in one launch: the planes of the
+    reference's -ujg dump, from the streams the reference wrote.  The group kernels skip the 4-segment records (the
+    8-segment ones cover the handoffs) to keep the emulated run short."""
+    imgs, streams_all, names = [], [], []
+    for name, source in extreme_leps():
+        if kernel != emu.KERNEL_WARP and "_t4." in name:
+            continue
+        lf = load_extreme_lep(name)
+        planes, streams = oracle_decode_planes(lf)
+        imgs.append(coef_image_from_lep(lf, [np.full_like(p, 77) for p in planes]))
+        streams_all.append(streams[:lf.nseg])
+        names.append((name, source))
+    st, _ = emu.decode_images(kernel, imgs, streams_all, grid_cap=3)
+    assert all(s == 0 for s in st), st
+    for (name, source), img in zip(names, imgs):
+        assert plane_hashes(img.planes) == EXTREMES[source]["plane_sha256"], name
+
+
+@pytest.mark.parametrize("kernel", KERNELS + GROUPS)
+@pytest.mark.parametrize("cfg", [
+    dict(ncmp=3, mcuh=6, mcuv=4, sf=((2, 2), (1, 1), (1, 1)), nseg=3, q16=True, max_cat=11),
+    dict(ncmp=3, mcuh=5, mcuv=5, sf=((2, 1), (1, 1), (1, 1)), nseg=2, q16=True, max_cat=11, density=0.9),
+    dict(ncmp=1, mcuh=8, mcuv=8, sf=((1, 1),), nseg=4, q16=True, max_cat=11, density=0.9),
+])
+def test_random_extreme_planes_decode_back(kernel, cfg):
+    """16-bit quantisers and magnitudes uniform over the categories 0..11 (the oracle codes every segment of these)."""
+    from lepton_b200 import CoefImage
+    rng = np.random.default_rng(1234)
+    img = random_coef_image(rng, **cfg)
+    ref = oracle_encode_image(img)
+    assert all(rc == 0 for rc, _, _ in ref)
+    out = CoefImage(ncmp=img.ncmp, mcuv=img.mcuv, bch=img.bch, bcv=img.bcv, qtables_zigzag=img.qtables_zigzag,
+                    planes=[np.full_like(p, -5) for p in img.planes], luma_y_start=img.luma_y_start)
+    st, nd = emu.decode_images(kernel, [out], [[s for _, s, _ in ref]])
+    assert all(s == 0 for s in st), st
+    assert nd == [n for _, _, n in ref]
+    for c in range(img.ncmp):
+        assert np.array_equal(out.planes[c], img.planes[c])

@@ -9,7 +9,8 @@ import pytest
 
 sys.path.insert(0, os.path.join(os.path.dirname(os.path.abspath(__file__)), "emu"))
 import emu  # noqa: E402
-from helpers import coef_image_from_lep, golden_leps, load_lep, oracle_decode_planes, oracle_encode_image, random_coef_image
+from helpers import (EXTREMES, coef_image_from_lep, extreme_jpegs, extreme_leps, golden_leps, load_extreme_lep, load_lep,
+                     oracle_decode_planes, oracle_encode_image, random_coef_image, read_golden)
 
 
 # range coder: 0 = range-only pass + parallel pieces + carry pass (the default), 1 = one serial chain per segment,
@@ -125,3 +126,62 @@ def test_zero_quantiser_status_both_directions():
                         planes=[np.zeros_like(p) for p in bad.planes], luma_y_start=bad.luma_y_start)
         st, _ = emu.decode_images(dk, [out], [[s for _, s, _ in good]])
         assert list(st) == [43, 43], (dk, st)
+
+
+def extreme_batch():
+    """Every image of the extreme corpus as the encoder gets it: the reference's .lep records (their geometry and splits,
+    planes from the oracle's decode) and the refused JPEGs (front end's planes).  -> images, per image a list of expected
+    (status, stream or None) per segment."""
+    from lepton_b200 import HostJpeg
+    imgs, want = [], []
+    for name, _ in extreme_leps():
+        lf = load_extreme_lep(name)
+        planes, streams = oracle_decode_planes(lf)
+        imgs.append(coef_image_from_lep(lf, planes))
+        want.append([(0, s) for s in streams[:lf.nseg]])
+    for n in extreme_jpegs():
+        if EXTREMES[n]["status_want"]:
+            img = HostJpeg(read_golden(EXTREMES[n]["path"])).coef_image()
+            imgs.append(img)
+            want.append([(rc, s if rc == 0 else None) for rc, s, _ in oracle_encode_image(img)])
+            assert EXTREMES[n]["status_want"] in [w[0] for w in want[-1]], n
+    return imgs, want
+
+
+@pytest.mark.parametrize("kernel", KERNELS)
+def test_extreme_corpus_batch_encode_matches_reference_streams(kernel):
+    """The extreme corpus in ONE batch (16-bit quantisers, category-11 magnitudes at every position, DC wrap, 4- and
+    8-segment records, two files the reference refuses): the reference's streams, and status 6 where it refused."""
+    imgs, want = extreme_batch()
+    got = emu.encode_images(imgs, grid_cap=3, kernel=kernel)
+    for k, (g, w) in enumerate(zip(got, want)):
+        assert [x[0] for x in g] == [s for s, _ in w], k
+        for (st, data, _), (_, ws) in zip(g, w):
+            if st == 0:
+                assert data == ws, k
+
+
+# coefficient regimes photos never reach: 16-bit quantisers, magnitudes uniform over the categories 0..11, DC over +-2047
+EXTREME_CFGS = [
+    dict(ncmp=3, mcuh=6, mcuv=4, sf=((2, 2), (1, 1), (1, 1)), nseg=3, q16=True, max_cat=11),
+    dict(ncmp=1, mcuh=8, mcuv=8, sf=((1, 1),), nseg=4, q16=True, max_cat=11, density=0.9),
+    dict(ncmp=3, mcuh=6, mcuv=4, sf=((2, 1), (1, 1), (1, 1)), nseg=3, max_cat=11),
+    dict(ncmp=1, mcuh=8, mcuv=8, sf=((1, 1),), nseg=8, max_cat=11, density=0.9),
+    dict(ncmp=3, mcuh=5, mcuv=4, sf=((1, 1), (1, 1), (1, 1)), nseg=2, q16=True, max_cat=11, dc_max=2047),
+    dict(ncmp=1, mcuh=6, mcuv=8, sf=((1, 1),), nseg=8, dc_max=2047),
+]
+
+
+@pytest.mark.parametrize("kernel", KERNELS)
+@pytest.mark.parametrize("cfg", EXTREME_CFGS)
+def test_random_extreme_planes_encode_vs_oracle(kernel, cfg):
+    """Status segment by segment as the oracle (6 where a coefficient or a DC residual cannot be coded), and the oracle's
+    stream and decision count for every segment it codes."""
+    rng = np.random.default_rng(4321)
+    img = random_coef_image(rng, **cfg)
+    ref = oracle_encode_image(img)
+    got = emu.encode_images([img], kernel=kernel)[0]
+    assert [g[0] for g in got] == [r[0] for r in ref]
+    for g, r in zip(got, ref):
+        if r[0] == 0:
+            assert (g[1], g[2]) == (r[1], r[2])

@@ -147,3 +147,51 @@ def test_huffman_encode_kernel_multi_segment_reference_files():
         scan, segs = emu.huffman_encode(job, HostJpeg(jpg).coef_image())
         assert [st for st, _ in segs] == [0] * job.nseg, (lep_name, segs)
         assert scan == jpg[off:off + n], lep_name
+
+
+# ---- the extreme corpus: Huffman codes up to 16 bits, category-11 magnitudes, runs of stuffed 0xFF bytes
+@pytest.mark.parametrize("sub_bits", [256, 1024, 4096])
+def test_extreme_jpegs_both_kernels_match_the_host_decoder(sub_bits):
+    """Serial and sub-sequence kernels give the host decoder's planes (pinned to the reference's -ujg dumps) and agree on
+    every row state.  The colour files are large enough that the sub-sequence kernels take them."""
+    from helpers import EXTREMES, extreme_jpegs, read_golden
+    names = extreme_jpegs()
+    jpegs = [read_golden(EXTREMES[n]["path"]) for n in names]
+    ser, _ = emu.huffman_decode(emu.HUFF_SERIAL, jpegs)
+    par, (iters, redo) = emu.huffman_decode(emu.HUFF_SUBSEQ, jpegs, sub_bits=sub_bits)
+    for n, s, p in zip(names, ser, par):
+        assert (s is None) == (p is None), n
+        if s is None:
+            assert not n.startswith("color"), n
+            continue
+        assert s["status"] == 0, n
+        for got, want in zip(s["planes"], s["host_planes"]):
+            assert np.array_equal(got, want), n
+        check_equal(p, s, n)
+    assert all(ser[names.index(n)] is not None for n in ("color420_long.jpg", "color444_long.jpg", "odd_rst.jpg"))
+    assert iters > 0
+    # with 256-bit sub-sequences, 16-bit codes resynchronise too slowly for some of these files: the serial kernel redoes
+    # them (same outputs, checked above)
+    assert redo == 0 or sub_bits == 256
+
+
+def test_huffman_encode_kernel_recreates_the_extreme_scans():
+    """lep_huffencode_kernel re-creates the scan of every extreme file byte for byte from the reference's .lep records:
+    16-bit codes, 0xFF stuffing, restart markers, and 4 and 8 segments whose handoffs carry extreme DC predictors."""
+    from helpers import EXTREMES, extreme_leps, read_golden
+    from lepton_b200 import HostJpeg, HostLep
+    multi = 0
+    for name, source in extreme_leps():
+        jpg = read_golden(EXTREMES[source]["path"])
+        hl = HostLep(read_golden("extremes/" + name))
+        assert hl.status == 0, hl.error
+        off, n = hl.scan_layout()
+        job = emu.henc_job(hl)
+        assert n > 0 and job.scan_bytes == n
+        img = HostJpeg(jpg).coef_image()
+        scan, segs = emu.huffman_encode(job, img)
+        assert [st for st, _ in segs] == [0] * job.nseg, (name, segs)
+        assert scan == jpg[off:off + n], name
+        assert hl.assemble(scan) == jpg, name
+        multi += job.nseg > 1
+    assert multi >= 5

@@ -10,7 +10,7 @@ import pytest
 sys.path.insert(0, os.path.join(os.path.dirname(os.path.abspath(__file__)), "emu"))
 import emu  # noqa: E402
 import lepfmt
-from helpers import GOLDEN, golden_leps
+from helpers import GOLDEN, extreme_leps, golden_leps, read_golden
 
 
 def split_lep(raw):
@@ -63,3 +63,12 @@ def test_random_stream_lengths_match_the_host_writer(seed):
             assert p.src_off == seen[p.id]
             seen[p.id] += p.len
         assert seen == [len(s) for s in streams]
+
+
+def test_extreme_corpus_leps_reassembled():
+    """The reference's .lep files of the extreme corpus (one, four and eight segments) from their own pieces."""
+    names = [n for n, _ in extreme_leps()]
+    raws = [read_golden("extremes/" + n) for n in names]
+    got = emu.mux_files([split_lep(r) for r in raws], grid=3)
+    for n, g, r in zip(names, got, raws):
+        assert g == r, n

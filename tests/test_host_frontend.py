@@ -8,7 +8,7 @@ import numpy as np
 import pytest
 
 import lepfmt
-from helpers import GOLDEN, MANIFEST, load_lep
+from helpers import EXTREMES, GOLDEN, MANIFEST, extreme_leps, load_extreme_lep, load_lep, plane_hashes, read_golden
 
 BASELINE_COMPLETE = ["android.jpg", "androidcrop.jpg", "androidcropoptions.jpg", "androidtrail.jpg", "colorswap.jpg",
                      "grayscale.jpg", "iphonecrop2.jpg", "trailingrst.jpg", "trailingrst2.jpg"]
@@ -310,3 +310,29 @@ def test_roundtripfail_fixture_host_halves():
     planes, _ = oracle_decode_planes(lf)
     back = hl.recode(planes)
     assert len(back) == len(d) and back != d
+
+
+@pytest.mark.parametrize("name,source", extreme_leps())
+def test_extreme_files_front_end_and_container_match_reference(name, source):
+    """The extreme corpus (16-bit DQT, 16-bit Huffman codes, category-11 magnitudes, restart intervals, partial MCUs):
+    the front end's planes equal the reference's -ujg dump, its thread-segment splits (with -minencodethreads=N for the
+    NAME_tN records) equal the reference's, and the container built around the reference's streams is its file."""
+    from lepton_b200 import HostJpeg
+    e = EXTREMES.get(name, {})
+    hj = HostJpeg(read_golden(EXTREMES[source]["path"]), min_threads=int(e["flags"][0].split("=")[1]) if e else 1)
+    assert hj.status == 0, hj.error
+    img = hj.coef_image()
+    assert plane_hashes(img.planes) == EXTREMES[source]["plane_sha256"], "Huffman-decoded planes differ from the reference's -ujg dump"
+    lf = load_extreme_lep(name)
+    assert list(img.luma_y_start) == [h.luma_y_start for h in lf.handoffs]
+    assert hj.write_lep(lepfmt.demux(lf.payload)[:lf.nseg]) == read_golden("extremes/" + name)
+
+
+def test_refused_extreme_files_are_parsed():
+    """The two files the reference refuses fail in the coder (status 6), not in the front end: their planes carry the
+    out-of-range values."""
+    from lepton_b200 import HostJpeg
+    img = HostJpeg(read_golden("extremes/dc_out_of_range.jpg")).coef_image()     # the planes are views into img's memory
+    assert img.planes[0][:, 49].max() == 1500
+    img = HostJpeg(read_golden("extremes/cat12.jpg")).coef_image()
+    assert np.abs(img.planes[0]).max() == 3000

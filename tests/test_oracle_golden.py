@@ -6,6 +6,7 @@ oracle/Makefile.ref); manifest.json holds sha256s of the coefficient planes from
  * oracle encode of those planes must reproduce the reference's segment streams byte for byte.
 The reference repository's own golden vector images/iphone16.lep (test_suite/test_16threads.sh) is checked in-container.
 """
+import hashlib
 import os
 
 import numpy as np
@@ -13,7 +14,8 @@ import pytest
 
 import lepfmt
 import oracle
-from helpers import GOLDEN, MANIFEST, geometry_of, golden_leps, load_lep, oracle_decode_planes, plane_hashes, segments_of
+from helpers import (EXTREMES, GOLDEN, MANIFEST, extreme_jpegs, extreme_leps, geometry_of, golden_leps, load_extreme_lep, load_lep,
+                     oracle_decode_planes, oracle_encode_image, plane_hashes, read_golden, segments_of)
 
 
 @pytest.mark.parametrize("name", golden_leps())
@@ -163,3 +165,97 @@ def test_oracle_vs_live_reference_on_a_large_fixture(tmp_path):
     for i, (y0, y1, last) in enumerate(segments_of(lf)):
         rc, s, _ = oracle.encode_segment(g, planes, y0, y1, last)
         assert rc == 0 and s == streams[i]
+
+
+# ---- the extreme corpus (tests/golden/make_extremes.py): coefficients, quantisers and Huffman codes at their limits
+@pytest.mark.parametrize("name,source", extreme_leps())
+def test_oracle_extremes_decode_to_the_reference_planes_and_reencode(name, source):
+    """Every reference-written .lep of the extreme corpus: the oracle decodes the reference's streams to the planes of the
+    reference's -ujg dump and re-encodes them to the same streams."""
+    raw = read_golden("extremes/" + name)
+    assert hashlib.md5(raw).hexdigest() == EXTREMES[name if name in EXTREMES else source]["lep_md5"]
+    lf = load_extreme_lep(name)
+    planes, streams = oracle_decode_planes(lf)
+    assert plane_hashes(planes) == EXTREMES[source]["plane_sha256"], "oracle decode != reference -ujg coefficient dump"
+    g, _, _ = geometry_of(lf)
+    for i, (y0, y1, last) in enumerate(segments_of(lf)):
+        rc, s, _ = oracle.encode_segment(g, planes, y0, y1, last)
+        assert rc == 0 and s == streams[i], "segment %d" % i
+
+
+def test_oracle_refuses_the_files_the_reference_refuses():
+    """dc_out_of_range (a DC beyond +-1024), dc_residual_long (a DC residual that round-trips but needs 12 bits) and cat12
+    (a 12-bit AC magnitude): the reference exits with COEFFICIENT_OUT_OF_RANGE; so does the oracle, on the front end's
+    planes."""
+    from lepton_b200 import HostJpeg
+    refused = [n for n in extreme_jpegs() if EXTREMES[n]["status_want"]]
+    assert sorted(refused) == ["cat12.jpg", "dc_out_of_range.jpg", "dc_residual_long.jpg"]
+    for n in refused:
+        assert EXTREMES[n]["exit_name"] == "COEFFICIENT_OUT_OF_RANGE" and EXTREMES[n]["status_want"] == 6
+        hj = HostJpeg(read_golden(EXTREMES[n]["path"]))
+        assert hj.status == 0, n
+        assert [r[0] for r in oracle_encode_image(hj.coef_image())] == [6], n
+
+
+# every place where the reference's arithmetic wraps, truncates or caps (oracle/lepton_oracle.c, "regime counters")
+REGIME_SITES = ["idct_int32_wrap", "idct_int16_pixel", "dc_est_int16", "edge_int16", "qdc_int16", "lak_uint32_wrap",
+                "sign_ctx_int16", "thr_ctx_mask", "thr_ctx_cap255", "bsr_cap1023", "len_mxm_cap11", "thr_so_sat127",
+                "adv_wrap_pos", "adv_wrap_neg", "ac_len11", "refuse_dc", "refuse_dc_len", "refuse_ac"]
+
+
+def test_extreme_corpus_reaches_every_wrap_and_cap_site():
+    """The oracle computes each wrapped or capped value exactly as well and counts where the two differ.  Coding the
+    extreme corpus has to reach every such site several times -- so a regenerated corpus cannot drift back into the range
+    photos live in, where a wrong cast, mask or division domain in the kernels would go unnoticed -- while the golden
+    photos reach almost none of them."""
+    from lepton_b200 import HostJpeg
+    assert sorted(oracle.regime_counts(reset=True)) == sorted(REGIME_SITES)
+    for n in extreme_jpegs():
+        oracle_encode_image(HostJpeg(read_golden(EXTREMES[n]["path"])).coef_image())
+    for name, _ in extreme_leps():
+        oracle_decode_planes(load_extreme_lep(name))
+    hit = oracle.regime_counts(reset=True)
+    assert all(hit[k] >= 3 for k in REGIME_SITES if not k.startswith("refuse")), hit
+    assert hit["refuse_dc"] >= 1 and hit["refuse_dc_len"] >= 1 and hit["refuse_ac"] >= 1, hit
+    for name in golden_leps():
+        oracle_decode_planes(load_lep(name))
+    photo = oracle.regime_counts(reset=True)
+    assert sum(photo[k] > 0 for k in REGIME_SITES) <= 3, photo
+
+
+def _div_trunc_small_f32(n, d):
+    """lep_predict.cuh div_trunc_small in numpy float32: __uint2float_rz of |n| and d (exact below 2^24), __frcp_rn
+    (the correctly rounded reciprocal), a round-to-nearest product truncated to an integer, one correction each way."""
+    a = np.abs(n).astype(np.int64)
+    rcp = np.float32(1) / d.astype(np.float32)
+    q = (a.astype(np.float32) * rcp).astype(np.int64)
+    rem = a - q * d
+    q = np.where(rem < 0, q - 1, q)
+    rem = np.where(rem < 0, rem + d, rem)
+    q = np.where(rem >= d, q + 1, q)
+    return np.where(n < 0, -q, q)
+
+
+def test_div_trunc_small_is_exact_over_the_callers_domain():
+    """div_trunc_small claims exact truncating division for |n| < 2^24, 1 <= d < 2^16 with a float reciprocal and one
+    correction step.  Its callers divide |avgmed| <= 2^18 (sums of eight int16 estimates) by q0 and |t| <= 2^18 (a 32-bit
+    sum shifted right by 13) by a quantiser.  Checked for every d < 2^16 at n = k d - 1, k d, k d + 1 for every multiple
+    k d up to 2^20, and at the multiples just below 2^24, both signs."""
+    for lo in range(1, 1 << 16, 4096):
+        d = np.arange(lo, min(lo + 4096, 1 << 16), dtype=np.int64)
+        for top in (1 << 20, 1 << 24):
+            kmax = top // d
+            kmin = np.maximum(kmax - 8, 1) if top == 1 << 24 else np.ones_like(d)
+            cnt = kmax - kmin + 1
+            dd = np.repeat(d, cnt)
+            k = np.repeat(kmin - np.cumsum(np.r_[0, cnt[:-1]]), cnt) + np.arange(cnt.sum())
+            n = (k * dd)[:, None] + np.array([-1, 0, 1])
+            dd = np.broadcast_to(dd[:, None], n.shape).ravel()
+            n = n.ravel()
+            keep = np.abs(n) < (1 << 24)
+            n, dd = n[keep], dd[keep]
+            for sgn in (1, -1):
+                got = _div_trunc_small_f32(sgn * n, dd)
+                want = sgn * (n // dd)
+                bad = np.nonzero(got != want)[0]
+                assert bad.size == 0, (int(sgn * n[bad[0]]), int(dd[bad[0]]), int(got[bad[0]]))

@@ -13,7 +13,9 @@ import numpy as np
 from PIL import Image
 
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
+sys.path.insert(0, os.path.dirname(os.path.abspath(__file__)))
 from lepton_b200 import HostJpeg  # noqa: E402
+from jpegwriter import BitWriter, canonical_codes, put_block  # noqa: E402
 
 ZZ2AL = [49, 50, 57, 58, 0, 51, 52, 1, 2, 59, 60, 3, 4, 5, 53, 54, 6, 7, 8, 9, 61, 62, 10, 11, 12, 13, 14, 55, 56, 15, 16,
          17, 18, 19, 20, 63, 21, 22, 23, 24, 25, 26, 27, 28, 29, 30, 31, 32, 33, 34, 35, 36, 37, 38, 39, 40, 41, 42, 43,
@@ -46,41 +48,8 @@ def dht_tables(segs):
             n = sum(bits)
             vals = list(s[p + 17:p + 17 + n])
             p += 17 + n
-            code = 0
-            k = 0
-            enc = {}
-            for ln in range(1, 17):
-                for _ in range(bits[ln - 1]):
-                    enc[vals[k]] = (code, ln)
-                    k += 1
-                    code += 1
-                code <<= 1
-            tabs[(tc, th)] = enc
+            tabs[(tc, th)] = canonical_codes(bits, vals)
     return tabs
-
-
-class BitWriter:
-    def __init__(self):
-        self.out = bytearray()
-        self.acc = 0
-        self.n = 0
-
-    def put(self, v, n):
-        if n == 0:
-            return
-        self.acc = (self.acc << n) | (v & ((1 << n) - 1))
-        self.n += n
-        while self.n >= 8:
-            b = (self.acc >> (self.n - 8)) & 255
-            self.out.append(b)
-            if b == 255:
-                self.out.append(0)
-            self.n -= 8
-        self.acc &= (1 << self.n) - 1
-
-    def pad(self):
-        while self.n & 7:
-            self.put(1, 1)
 
 
 def make(w, h, sub, q, rst, name):
@@ -128,30 +97,7 @@ def make(w, h, sub, q, rst, name):
                     bw.out += bytes([0xFF, 0xD0 + (nrst & 7)])
                     nrst += 1
                     last = 0
-                blk = P[by * bch + bx]
-                z = [int(blk[ZZ2AL[k]]) for k in range(64)]
-                d = z[0] - last
-                last = z[0]
-                s = abs(d).bit_length()
-                bw.put(*dc[s])
-                bw.put(d if d > 0 else d - 1 + (1 << s), s)
-                end = 63
-                while end > 0 and z[end] == 0:
-                    end -= 1
-                run = 0
-                for k in range(1, end + 1):
-                    if z[k] == 0:
-                        run += 1
-                        continue
-                    while run >= 16:
-                        bw.put(*ac[0xF0])
-                        run -= 16
-                    s = abs(z[k]).bit_length()
-                    bw.put(*ac[(run << 4) | s])
-                    bw.put(z[k] if z[k] > 0 else z[k] - 1 + (1 << s), s)
-                    run = 0
-                if end != 63:
-                    bw.put(*ac[0])
+                last = put_block(bw, [int(v) for v in P[by * bch + bx][ZZ2AL]], last, dc, ac)
                 cnt += 1
         bw.pad()
         out += bw.out
