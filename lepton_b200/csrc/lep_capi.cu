@@ -81,6 +81,7 @@ struct lepb200_ctx {
     DevBuf d_gather, d_lit;                // device container assembly: piece list, literal bytes (file headers + trailers)
     HostBuf h_lit;
     DevBuf d_rc_ck, d_rc_digits;           // parallel range coder: checkpoints of the range-only pass, deferred-carry digits
+    DevBuf d_rc_ovf, d_rc_redo;            // streams longer than their slot (both range coder forms); serial form: segments it codes again
     HostBuf h_henc_out, h_henc_segs, h_henc_desc;
     cudaEvent_t status_ev = nullptr;       // parts mode: the D2H of the decode batch's segment records, queued ahead of the part copies
     bool status_queued = false;
@@ -263,7 +264,11 @@ int build_batch(lepb200_ctx* ctx, const lepb200_image* images, int nimages, bool
             size_t nb = segment_blocks(im, sd.min_y, sd.max_y, sd.is_last);
             ctx->seg_blocks.push_back(nb);
             if (encode) {
-                size_t cap = align_up(nb * 64 + 4096, 256);   // 64 B/block is > 1.5x what q=100 photos need; overflow is reported, never silent
+                // 64 B/block is > 1.5x what q=100 photos need.  Dense noise needs more (up to about 7/8 byte per decision):
+                // such a stream moves to the overflow arena, sized from the exact length (parallel range coder, see
+                // lep_digit_offsets_kernel) or from a proven bound when the serial coder codes the segment again
+                // (rerun_overflowed_serial).  No stream is ever cut short.
+                size_t cap = align_up(nb * 64 + 4096, 256);
                 sd.stream = stream_total; sd.cap = (uint32_t)cap;
                 stream_total += cap;
                 sd.tokens = 0; sd.tok_cap = 0;                    // assigned on the device by the counting pre-pass ...
@@ -405,7 +410,7 @@ void lepb200_destroy(lepb200_ctx* ctx) {
     if (!ctx) return;
     cudaSetDevice(ctx->device);
     cudaStreamSynchronize(ctx->stream);
-    for (DevBuf* b : {&ctx->d_henc_out, &ctx->d_henc_imgs, &ctx->d_henc_segs, &ctx->d_henc_tabs, &ctx->d_huff, &ctx->d_hjobs, &ctx->d_htabs, &ctx->d_hrows, &ctx->d_hpar, &ctx->d_planes, &ctx->d_streams, &ctx->d_tokens, &ctx->d_dense, &ctx->d_images, &ctx->d_segs, &ctx->d_order, &ctx->d_counter, &ctx->d_models, &ctx->d_rows, &ctx->d_rc_ck, &ctx->d_rc_digits, &ctx->d_gather, &ctx->d_lit})
+    for (DevBuf* b : {&ctx->d_henc_out, &ctx->d_henc_imgs, &ctx->d_henc_segs, &ctx->d_henc_tabs, &ctx->d_huff, &ctx->d_hjobs, &ctx->d_htabs, &ctx->d_hrows, &ctx->d_hpar, &ctx->d_planes, &ctx->d_streams, &ctx->d_tokens, &ctx->d_dense, &ctx->d_images, &ctx->d_segs, &ctx->d_order, &ctx->d_counter, &ctx->d_models, &ctx->d_rows, &ctx->d_rc_ck, &ctx->d_rc_digits, &ctx->d_rc_ovf, &ctx->d_rc_redo, &ctx->d_gather, &ctx->d_lit})
         b->release();
     for (HostBuf* b : {&ctx->h_segs, &ctx->h_dense, &ctx->h_stage, &ctx->h_hjobs, &ctx->h_hpar}) b->release();
     cudaEventDestroy(ctx->ev0);
@@ -423,7 +428,7 @@ void lepb200_release_device_buffers(lepb200_ctx* ctx) {
     cudaSetDevice(ctx->device);
     cudaStreamSynchronize(ctx->stream);
     cudaStreamSynchronize(ctx->copy_stream);
-    for (DevBuf* b : {&ctx->d_henc_out, &ctx->d_henc_imgs, &ctx->d_henc_segs, &ctx->d_henc_tabs, &ctx->d_huff, &ctx->d_hjobs, &ctx->d_htabs, &ctx->d_hrows, &ctx->d_hpar, &ctx->d_planes, &ctx->d_streams, &ctx->d_tokens, &ctx->d_dense, &ctx->d_images, &ctx->d_segs, &ctx->d_order, &ctx->d_counter, &ctx->d_models, &ctx->d_rows, &ctx->d_rc_ck, &ctx->d_rc_digits, &ctx->d_gather, &ctx->d_lit})
+    for (DevBuf* b : {&ctx->d_henc_out, &ctx->d_henc_imgs, &ctx->d_henc_segs, &ctx->d_henc_tabs, &ctx->d_huff, &ctx->d_hjobs, &ctx->d_htabs, &ctx->d_hrows, &ctx->d_hpar, &ctx->d_planes, &ctx->d_streams, &ctx->d_tokens, &ctx->d_dense, &ctx->d_images, &ctx->d_segs, &ctx->d_order, &ctx->d_counter, &ctx->d_models, &ctx->d_rows, &ctx->d_rc_ck, &ctx->d_rc_digits, &ctx->d_rc_ovf, &ctx->d_rc_redo, &ctx->d_gather, &ctx->d_lit})
         b->release();
     ctx->have_batch = ctx->launched = false;
 }
@@ -770,11 +775,14 @@ int lepb200_encode_launch_rangecode(lepb200_ctx* ctx) {
         else lep_rangepass_kernel<false><<<(nseg + RCT_THREADS - 1) / RCT_THREADS, RCT_THREADS, RCT_SMEM_TABLE_BYTES, ctx->stream>>>(ds, nseg, dord, dtok, dck);
         CK(cudaGetLastError());
         unsigned long long* d_total = reinterpret_cast<unsigned long long*>(static_cast<uint8_t*>(ctx->d_counter.p) + 128);
-        lep_digit_offsets_kernel<<<1, 1024, 0, ctx->stream>>>(ds, nseg, d_total);
+        lep_digit_offsets_kernel<<<1, 1024, 0, ctx->stream>>>(ds, nseg, d_total, d_total + 1);
         CK(cudaGetLastError());
-        unsigned long long total_digits = 0;
-        CK(cudaMemcpyAsync(&total_digits, d_total, sizeof(total_digits), cudaMemcpyDeviceToHost, ctx->stream));
+        // [0] digits, [1] bytes of the overflow arena (streams longer than their slot; 0 for photo batches) -- one copy, one sync
+        unsigned long long totals[2] = {0, 0};
+        CK(cudaMemcpyAsync(totals, d_total, sizeof(totals), cudaMemcpyDeviceToHost, ctx->stream));
         CK(cudaStreamSynchronize(ctx->stream));
+        const unsigned long long total_digits = totals[0];
+        if (totals[1]) CK(ctx->d_rc_ovf.reserve((size_t)totals[1]));
         if (trace) cudaEventRecord(te[1], ctx->stream);
         CK(ctx->d_rc_digits.reserve((size_t)total_digits * 4 + 256));
         CK(cudaMemsetAsync(ctx->d_rc_digits.p, 0, (size_t)total_digits * 4, ctx->stream));
@@ -782,7 +790,8 @@ int lepb200_encode_launch_rangecode(lepb200_ctx* ctx) {
         lep_rangepiece_kernel<<<dim3(8, (unsigned)nseg), RCP_THREADS, 0, ctx->stream>>>(ds, nseg, dtok, dck, ddig);
         CK(cudaGetLastError());
         if (trace) cudaEventRecord(te[2], ctx->stream);
-        lep_rangenorm_kernel<<<(nseg + RCN_WARPS - 1) / RCN_WARPS, RCN_WARPS * 32, 0, ctx->stream>>>(ds, nseg, dord, ddig);
+        lep_rangenorm_kernel<<<(nseg + RCN_WARPS - 1) / RCN_WARPS, RCN_WARPS * 32, 0, ctx->stream>>>(ds, nseg, dord, ddig,
+                                                                                                       static_cast<uint8_t*>(ctx->d_rc_ovf.p));
         CK(cudaGetLastError());
         if (trace) {
             cudaEventRecord(te[3], ctx->stream);
@@ -810,6 +819,42 @@ int lepb200_encode_launch(lepb200_ctx* ctx) {
     return r ? r : lepb200_encode_launch_rangecode(ctx);
 }
 
+// Serial range coder (rc_mode 0): it learns a stream's length only by writing it, so a stream longer than its slot comes
+// back with ST_OUT_OVERFLOW (kernel A's token overflow, ntok > tok_cap, is the other source of that status and stays an
+// error).  Its tokens are still in the arena: lep_rangecode_kernel codes those segments again, alone, into the overflow
+// arena, with a capacity no stream can reach.  Bound: before every decision the range is normalised (>= 128), and the
+// sub-range kept is >= 1 (split >= 1, and split <= 1 + (range - 1) * 255 / 256 < range), so a decision shifts at most 7 bits;
+// with the marker bit and the 32 stop decisions a segment shifts T <= 7 (ntok + 33) bits, and writes at most
+// (T - 16) / 8 bytes plus the zero byte of the stop rule.  hs (the segment records, fetched) is updated in place.
+static size_t serial_stream_bound(uint32_t ntok) { return align_up((7ull * ((unsigned long long)ntok + 33) + 8) / 8 + 2, 256); }
+static int rerun_overflowed_serial(lepb200_ctx* ctx, SegDesc* hs, int nseg) {
+    if (ctx->rc_mode == 1) return LEPB200_OK;
+    std::vector<int> redo;
+    size_t total = 0;
+    for (int s = 0; s < nseg; ++s)
+        if (hs[s].status == ST_OUT_OVERFLOW && hs[s].ntok <= hs[s].tok_cap) { redo.push_back(s); total += serial_stream_bound(hs[s].ntok); }
+    if (redo.empty()) return LEPB200_OK;
+    CK(ctx->d_rc_ovf.reserve(total));
+    CK(ctx->d_rc_redo.reserve(sizeof(int) * redo.size()));
+    size_t off = 0;
+    for (int s : redo) {
+        hs[s].stream = (unsigned long long)(uintptr_t)ctx->d_rc_ovf.p + off;
+        hs[s].cap = (uint32_t)serial_stream_bound(hs[s].ntok);
+        hs[s].status = ST_OK; hs[s].len = 0;
+        off += hs[s].cap;
+    }
+    const int n = (int)redo.size();
+    CK(cudaMemcpyAsync(ctx->d_segs.p, hs, sizeof(SegDesc) * nseg, cudaMemcpyHostToDevice, ctx->stream));
+    CK(cudaMemcpyAsync(ctx->d_rc_redo.p, redo.data(), sizeof(int) * n, cudaMemcpyHostToDevice, ctx->stream));
+    lep_rangecode_kernel<<<(n + RC_THREADS - 1) / RC_THREADS, RC_THREADS, 0, ctx->stream>>>(
+        static_cast<SegDesc*>(ctx->d_segs.p), n, static_cast<const int*>(ctx->d_rc_redo.p), static_cast<const uint16_t*>(ctx->d_tokens.p));
+    CK(cudaGetLastError());
+    ctx->launches += 1;
+    CK(cudaMemcpyAsync(hs, ctx->d_segs.p, sizeof(SegDesc) * nseg, cudaMemcpyDeviceToHost, ctx->stream));
+    CK(cudaStreamSynchronize(ctx->stream));
+    return LEPB200_OK;
+}
+
 int lepb200_encode_fetch(lepb200_ctx* ctx, lepb200_stream* out) {
     if (!ctx || !ctx->launched || !ctx->is_encode || !out) { if (ctx) ctx->err = "encode_fetch without encode_launch"; return LEPB200_ERR_INVALID; }
     CK(cudaSetDevice(ctx->device));
@@ -819,6 +864,7 @@ int lepb200_encode_fetch(lepb200_ctx* ctx, lepb200_stream* out) {
     CK(cudaMemcpyAsync(hs, ctx->d_segs.p, sizeof(SegDesc) * nseg, cudaMemcpyDeviceToHost, ctx->stream));
     CK(cudaStreamSynchronize(ctx->stream));
     CK(cudaEventElapsedTime(&ctx->last_ms, ctx->ev0, ctx->ev1));
+    if (const int r = rerun_overflowed_serial(ctx, hs, nseg)) return r;
     // dense layout of the produced streams
     unsigned long long* offs = reinterpret_cast<unsigned long long*>(hs + nseg);
     size_t total = 0;
@@ -863,6 +909,7 @@ int lepb200_encode_fetch_files(lepb200_ctx* ctx, const lepb200_buffer* headers, 
     CK(cudaMemcpyAsync(hs, ctx->d_segs.p, sizeof(SegDesc) * nseg, cudaMemcpyDeviceToHost, ctx->stream));
     CK(cudaStreamSynchronize(ctx->stream));
     CK(cudaEventElapsedTime(&ctx->last_ms, ctx->ev0, ctx->ev1));
+    if (const int r = rerun_overflowed_serial(ctx, hs, nseg)) return r;
     // literals: header + 4 trailer bytes per image, 16-byte aligned
     size_t lit_total = 0;
     std::vector<size_t> lit_off(nimg);

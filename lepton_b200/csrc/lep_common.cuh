@@ -111,6 +111,8 @@ struct SegDesc {
     uint32_t tok_cap;
     uint32_t total_shift;            // encode, parallel range coder: bits the coder shifted out over the whole segment (incl. marker and stop bits)
     unsigned long long digits;       // encode, parallel range coder: offset of the segment's 16-bit digits in the digit arena
+    unsigned long long ovf;          // encode, parallel range coder: 1 + offset of the segment's stream in the overflow arena when
+                                     // the stream does not fit `cap` (lep_digit_offsets_kernel), 0 when it stays where it is
 };
 
 enum : int32_t { ST_OK = 0, ST_ASSERT = 1, ST_COEF_RANGE = 6, ST_STREAM_INCONSISTENT = 7, ST_OUT_OVERFLOW = 100 };

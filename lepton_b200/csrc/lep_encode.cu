@@ -606,7 +606,9 @@ __device__ __forceinline__ void rc_store(RcState& w, uint32_t byte) {
 __device__ __forceinline__ void rc_emit_slow(RcState& w, uint32_t b, bool carry) {
     if (carry) {
         if (w.cache == 0xff || w.cache < 0) {
-            long x = (long)w.mpos - 1;
+            // bytes past the capacity were never stored: the walk starts inside the stream (the segment reports overflow
+            // and is coded again into a larger buffer, so the bytes it changes here do not matter, only that it stays in bounds)
+            long x = (long)min(w.mpos, w.cap) - 1;
             while (x >= 0 && w.buf[x] == 0xff) { w.buf[x] = 0; --x; }
             if (x >= 0) w.buf[x] += 1;
             if (w.cache == 0xff) w.cache = 0;
@@ -870,23 +872,48 @@ lep_rangepass_kernel(SegDesc* __restrict__ segs, int nseg, const int* __restrict
     sd.total_shift = S;
 }
 
-// exclusive scan of the digit counts -> digit offsets; total in *total_out.  Single CTA (cf. lep_token_offsets_kernel).
-__global__ void lep_digit_offsets_kernel(SegDesc* __restrict__ segs, int nseg, unsigned long long* __restrict__ total_out) {
-    __shared__ unsigned long long sums[1024];
+// Stream bytes of a segment that shifted T bits in all: L = (T - 16) >> 3 leave the window (boolwriter.hh:88), plus at most
+// the one zero byte of the stop rule.  A segment whose L + 1 bytes may not fit below its capacity (the overflow check of
+// lep_rangenorm_kernel is len >= cap) gets a slot of this size in the overflow arena instead.
+__device__ __forceinline__ unsigned long long rc_overflow_bytes(const SegDesc& sd) {
+    const unsigned long long T = sd.total_shift, L = T >= 16 ? (T - 16) >> 3 : 0;
+    return L + 1 >= sd.cap ? (L + 2 + 255) & ~255ull : 0ull;
+}
+
+// exclusive scans of the digit counts -> digit offsets (total in *total_out), and of the overflow slots -> SegDesc::ovf (+
+// the capacity of the slot; total in *ovf_total_out, 0 for every batch whose streams fit their capacity).  Without
+// ovf_total_out the caller has no overflow arena: no stream moves, and one that does not fit reports ST_OUT_OVERFLOW.
+// Single CTA (cf. lep_token_offsets_kernel).
+__global__ void lep_digit_offsets_kernel(SegDesc* __restrict__ segs, int nseg, unsigned long long* __restrict__ total_out,
+                                         unsigned long long* __restrict__ ovf_total_out = nullptr) {
+    const bool grow = ovf_total_out != nullptr;
+    __shared__ unsigned long long sums[1024], osums[1024];
     const int t = threadIdx.x, per = (nseg + 1023) / 1024;
     const int b = t * per, e = min(nseg, b + per);
-    unsigned long long s = 0;
-    for (int i = b; i < e; ++i) s += ((unsigned long long)segs[i].total_shift + 8 + 15) / 16 + 2;
+    unsigned long long s = 0, o = 0;
+    for (int i = b; i < e; ++i) { s += ((unsigned long long)segs[i].total_shift + 8 + 15) / 16 + 2; o += grow ? rc_overflow_bytes(segs[i]) : 0ull; }
     sums[t] = s;
+    osums[t] = o;
     __syncthreads();
     if (t == 0) {
-        unsigned long long run = 0;
-        for (int i = 0; i < 1024; ++i) { unsigned long long v = sums[i]; sums[i] = run; run += v; }
+        unsigned long long run = 0, orun = 0;
+        for (int i = 0; i < 1024; ++i) {
+            unsigned long long v = sums[i], w = osums[i];
+            sums[i] = run; run += v;
+            osums[i] = orun; orun += w;
+        }
         *total_out = run;
+        if (grow) *ovf_total_out = orun;
     }
     __syncthreads();
-    unsigned long long off = sums[t];
-    for (int i = b; i < e; ++i) { segs[i].digits = off; off += ((unsigned long long)segs[i].total_shift + 8 + 15) / 16 + 2; }
+    unsigned long long off = sums[t], ooff = osums[t];
+    for (int i = b; i < e; ++i) {
+        SegDesc& sd = segs[i];
+        sd.digits = off; off += ((unsigned long long)sd.total_shift + 8 + 15) / 16 + 2;
+        const unsigned long long ob = grow ? rc_overflow_bytes(sd) : 0ull;
+        sd.ovf = ob ? ooff + 1 : 0;
+        if (ob) { sd.cap = (uint32_t)ob; ooff += ob; }
+    }
 }
 
 // (2) one thread per piece of RC_PIECE tokens: grid.y = segment, pieces strided over grid.x * blockDim.x threads.
@@ -968,7 +995,8 @@ lep_rangepiece_kernel(const SegDesc* __restrict__ segs, int nseg, const uint16_t
 // position j when a = generate | propagate, b = generate).  Lane l holds digit base + l; carries run from lane 31 to lane 0.
 constexpr int RCN_WARPS = 4;
 __global__ void __launch_bounds__(RCN_WARPS * 32)
-lep_rangenorm_kernel(SegDesc* __restrict__ segs, int nseg, const int* __restrict__ order, const uint32_t* __restrict__ digit_base) {
+lep_rangenorm_kernel(SegDesc* __restrict__ segs, int nseg, const int* __restrict__ order, const uint32_t* __restrict__ digit_base,
+                     uint8_t* __restrict__ ovf_base = nullptr) {
     const int t = blockIdx.x * RCN_WARPS + (threadIdx.x >> 5);
     const int lane = threadIdx.x & 31;
     if (t >= nseg) return;
@@ -978,7 +1006,8 @@ lep_rangenorm_kernel(SegDesc* __restrict__ segs, int nseg, const int* __restrict
     const uint32_t L = T >= 16 ? (T - 16) >> 3 : 0;                    // bytes that leave the window (boolwriter.hh:88)
     const uint32_t nd = (T + 8 + 15) / 16;
     const uint32_t* dig = digit_base + sd.digits;
-    uint8_t* buf = reinterpret_cast<uint8_t*>(sd.stream);
+    // a stream longer than its slot goes to the overflow arena (lep_digit_offsets_kernel sized the slot and set cap)
+    uint8_t* buf = sd.ovf ? ovf_base + (sd.ovf - 1) : reinterpret_cast<uint8_t*>(sd.stream);
     const uint32_t cap = sd.cap;
     uint32_t g_prev = 0, c_prev = 0, last = 0;
     const int nbatch = (int)((nd + 31) / 32);
@@ -1012,6 +1041,7 @@ lep_rangenorm_kernel(SegDesc* __restrict__ segs, int nseg, const int* __restrict
     if (L > 0 && (last & 0xe0) == 0xc0) { if (lane == 0 && len < cap) buf[len] = 0; ++len; }     // boolwriter.cc:32-34
     if (lane == 0) {
         sd.len = len;
+        sd.stream = (unsigned long long)(uintptr_t)buf;               // where lep_compact_kernel and lep_gather_kernel find it
         if (len >= cap) sd.status = ST_OUT_OVERFLOW;
     }
 }

@@ -119,6 +119,11 @@ typedef struct {
     uint32_t low, range; int count; size_t pos; uint8_t *buf; size_t cap; int overflow;
 } BoolWriter;
 
+/* bool-coder regime counters (lo_bool_counts): bytes a carry changes (the 0xff bytes it turns into zeros, plus the byte it
+ * increments) -- the longest such walk and the number of walks of 64 bytes or more -- and the streams that end with the
+ * extra zero byte of vpx_stop_encode */
+static uint64_t g_bw_walk_max, g_bw_walk_long, g_bw_stop_zero;
+
 static void bw_write(BoolWriter *w, int bit, int prob) {
     uint32_t split = 1 + (((w->range - 1) * (uint32_t)prob) >> 8);
     uint32_t range = split, low = w->low;
@@ -133,6 +138,9 @@ static void bw_write(BoolWriter *w, int bit, int prob) {
             long x = (long)w->pos - 1;
             while (x >= 0 && w->buf[x] == 0xff) { w->buf[x] = 0; x--; }
             w->buf[x] += 1;
+            const uint64_t walk = (uint64_t)((long)w->pos - x);
+            if (walk > g_bw_walk_max) g_bw_walk_max = walk;
+            if (walk >= 64) ++g_bw_walk_long;
         }
         if (w->pos + 2 >= w->cap) { w->overflow = 1; w->pos = 0; }
         w->buf[w->pos++] = (uint8_t)(low >> (24 - offset));
@@ -150,7 +158,7 @@ static void bw_start(BoolWriter *w, uint8_t *buf, size_t cap) {
 }
 static void bw_stop(BoolWriter *w) {
     for (int i = 0; i < 32; i++) bw_write(w, 0, 128);
-    if ((w->buf[w->pos - 1] & 0xe0) == 0xc0) w->buf[w->pos++] = 0;
+    if ((w->buf[w->pos - 1] & 0xe0) == 0xc0) { w->buf[w->pos++] = 0; ++g_bw_stop_zero; }
 }
 
 /* src/vp8/decoder/boolreader.hh:184-258,376-416, boolreader.cc:26-35.  The reference refills a 64-bit
@@ -901,6 +909,24 @@ int lo_decode_segment(const lo_geometry *g, int16_t *const planes[3], int min_y,
     codec_free(&c);
     return e;
 }
+
+/* The bool coder alone: vpx_start_encode, one vpx_write per token, vpx_stop_encode.  Token k = prob | bit << 8 (the
+ * layout kernel A writes).  Returns 0, or LO_OUTPUT_OVERFLOW when the stream (plus 2 bytes of room) does not fit `cap`;
+ * then *out_len = 0 and the bytes in `out` are meaningless. */
+int lo_bool_encode(const uint16_t *tokens, size_t n, uint8_t *out, size_t cap, size_t *out_len) {
+    *out_len = 0;
+    if (cap < 8) return LO_OUTPUT_OVERFLOW;
+    BoolWriter w;
+    bw_start(&w, out, cap);
+    for (size_t i = 0; i < n && !w.overflow; ++i) bw_write(&w, (tokens[i] >> 8) & 1, tokens[i] & 0xff);
+    if (w.overflow) return LO_OUTPUT_OVERFLOW;
+    bw_stop(&w);
+    if (w.overflow) return LO_OUTPUT_OVERFLOW;
+    *out_len = w.pos;
+    return 0;
+}
+void lo_bool_counts(uint64_t out[3]) { out[0] = g_bw_walk_max; out[1] = g_bw_walk_long; out[2] = g_bw_stop_zero; }
+void lo_bool_counts_reset(void) { g_bw_walk_max = g_bw_walk_long = g_bw_stop_zero = 0; }
 
 size_t lo_model_bytes(void) { return sizeof(Model); }
 

@@ -94,6 +94,31 @@ def decode_segment(g: Geometry, planes, min_y, max_y, is_last, stream: bytes):
     return rc, nd.value
 
 
+def bool_encode(tokens, cap=None):
+    """The bool coder alone over `tokens` (uint16: prob | bit << 8), marker bit and stop rule included.
+    -> (exit_code, stream bytes); exit code 100 when the stream does not fit `cap` bytes (default: always fits)."""
+    L = lib()
+    L.lo_bool_encode.argtypes = [ctypes.c_void_p, ctypes.c_size_t, ctypes.c_void_p, ctypes.c_size_t, ctypes.POINTER(ctypes.c_size_t)]
+    L.lo_bool_encode.restype = ctypes.c_int
+    t = np.ascontiguousarray(tokens, dtype=np.uint16)
+    cap = cap or len(t) + 64          # a decision shifts at most 7 bits: < 1 byte each
+    out = np.zeros(cap, dtype=np.uint8)
+    n = ctypes.c_size_t(0)
+    rc = L.lo_bool_encode(t.ctypes.data if len(t) else None, len(t), out.ctypes.data, cap, ctypes.byref(n))
+    return rc, out[:n.value].tobytes()
+
+
+def bool_counts(reset=False):
+    """Bool-coder regimes reached since the last reset, by bool_encode and encode_segment alike: longest carry walk
+    (bytes a carry changed), carry walks of 64 bytes or more, streams that ended with the extra zero byte of the stop rule."""
+    L = lib()
+    out = (ctypes.c_uint64 * 3)()
+    L.lo_bool_counts(out)
+    if reset:
+        L.lo_bool_counts_reset()
+    return dict(walk_max=int(out[0]), walks_64=int(out[1]), stop_zero=int(out[2]))
+
+
 def regime_counts(reset=False):
     """{site: count} since the last reset: how often each place where the reference's arithmetic wraps, truncates or
     caps (int32 IDCT, int16 pixels and edges, uint32 Lakhani sum, context masks and caps, DC wrap, status 6) produced a

@@ -71,6 +71,10 @@ inline Cta g_cta;
 inline Lane* g_cur = nullptr;
 inline unsigned long long g_progress = 0;       // arrivals + exits: a wait loop that sees no progress for long is a deadlock
 inline Dim3 g_block_idx, g_block_dim, g_grid_dim;
+// schedule: false = CTAs in order and, inside a CTA, thread 0 first (each runs until it waits or returns); true = the
+// last CTA first and the threads of a CTA from the last one down.  A kernel that is right only because of the order in
+// which its threads touch shared data gives different results under the two.
+inline bool g_reverse = false;
 
 extern "C" void emu_ctx_switch(void** from_sp, void* to_sp);
 #if defined(__x86_64__)
@@ -108,7 +112,8 @@ inline void yield() {
     const int n = c.nthreads;
     int i = (int)(from - c.lanes.data());
     for (int k = 0; k < n; ++k) {
-        i = i + 1 == n ? 0 : i + 1;
+        if (g_reverse) i = i == 0 ? n - 1 : i - 1;
+        else i = i + 1 == n ? 0 : i + 1;
         if (!c.lanes[i].done) {
             if (&c.lanes[i] == from) return;           // everybody else is gone: keep going (a wait loop will re-check)
             g_cur = &c.lanes[i];
@@ -193,7 +198,8 @@ inline void launch(unsigned grid, unsigned block, void (*body)(void*), void* arg
     }
     g_block_dim.x = block; g_block_dim.y = g_block_dim.z = 1;
     g_grid_dim.x = grid; g_grid_dim.y = g_grid_dim.z = 1;
-    for (unsigned b = 0; b < grid; ++b) {
+    for (unsigned bb = 0; bb < grid; ++bb) {
+        const unsigned b = g_reverse ? grid - 1 - bb : bb;
         g_block_idx.x = b;
         c.nthreads = (int)block; c.live = (int)block; c.sync_gen = 0; c.sync_arrived = 0;
         c.body = body; c.arg = arg;
@@ -212,7 +218,7 @@ inline void launch(unsigned grid, unsigned block, void (*body)(void*), void* arg
             l.sp = sp;
         }
         for (unsigned t = block; t < ((block + 31) / 32) * 32; ++t) { c.warps[t >> 5].exited++; c.warps[t >> 5].exited_mask |= 1u << (t & 31); }      // lanes of a partial warp that do not exist
-        g_cur = &c.lanes[0];
+        g_cur = &c.lanes[g_reverse ? block - 1 : 0];
         emu_ctx_switch(&c.main_sp, g_cur->sp);
         if (c.live != 0) { fprintf(stderr, "warp emulator: CTA %u stopped with %d threads parked (deadlock)\n", b, c.live); abort(); }
     }

@@ -90,15 +90,17 @@ def decode_images(kernel, images, streams, grid_cap=0):
 ENC_KERNEL_A = 0
 
 
-def encode_images(images, grid_cap=0, kernel=0):
-    """Same contract as LeptonB200Codec.encode_images: per image a list of (status, bytes, ndecisions) per segment."""
+def encode_images(images, grid_cap=0, kernel=0, tok_caps=False):
+    """Same contract as LeptonB200Codec.encode_images: per image a list of (status, bytes, ndecisions) per segment.
+    tok_caps=True: returns (that list, token bound of every segment as the count pre-pass sized it)."""
     from lepton_b200.codec import _Image, _Stream
     n = sum(im.nseg for im in images)
     cim = (_Image * len(images))(*[im.to_c() for im in images])
     out = (_Stream * n)()
-    cap = sum(im.blocks() for im in images) * 64 + 8192 * n
+    cap = sum(im.blocks() for im in images) * 128 + 8192 * n          # a stream holds < 1 byte per decision
     arena = (ctypes.c_uint8 * cap)()
-    rc = lib().emu_encode_images(int(kernel), int(grid_cap), cim, len(images), out, arena, ctypes.c_size_t(cap))
+    tc = (ctypes.c_uint32 * n)()
+    rc = lib().emu_encode_images(int(kernel), int(grid_cap), cim, len(images), out, arena, ctypes.c_size_t(cap), tc)
     if rc != 0:
         raise RuntimeError("emu_encode_images failed with %d" % rc)
     res, k = [], 0
@@ -109,7 +111,34 @@ def encode_images(images, grid_cap=0, kernel=0):
             segs.append((o.status, ctypes.string_at(o.data, o.len) if o.len else b"", int(o.ndecisions)))
             k += 1
         res.append(segs)
-    return res
+    return (res, list(tc)) if tok_caps else res
+
+
+def range_code(kernel, streams, caps, reverse=False):
+    """Kernel B alone (emu_range_code): streams = list of uint16 token arrays (prob | bit << 8), caps = stream slot of each.
+    kernel 0 / 2 = the parallel range coder (cp.async / register token feed), 1 = the serial one.  reverse runs CTAs and
+    threads in reverse order.  -> (per segment (status, bytes, moved to the overflow arena), canary bytes that changed)."""
+    toks = [np.ascontiguousarray(t, dtype=np.uint16) for t in streams]
+    n = len(toks)
+    flat = np.concatenate(toks) if n and sum(len(t) for t in toks) else np.zeros(1, np.uint16)
+    nt = (ctypes.c_uint32 * n)(*[len(t) for t in toks])
+    cp = (ctypes.c_uint32 * n)(*[int(c) for c in caps])
+    st = (ctypes.c_int32 * n)()
+    ln = (ctypes.c_uint32 * n)()
+    mv = (ctypes.c_uint8 * n)()
+    out_cap = sum(len(t) for t in toks) + 64 * n + 64
+    out = (ctypes.c_uint8 * out_cap)()
+    bad = ctypes.c_uint64(0)
+    f = lib().emu_range_code
+    f.restype = ctypes.c_int
+    rc = f(int(kernel), int(bool(reverse)), n, flat.ctypes.data_as(ctypes.c_void_p), nt, cp, st, ln, mv, out, ctypes.c_size_t(out_cap), ctypes.byref(bad))
+    if rc != 0:
+        raise RuntimeError("emu_range_code failed with %d" % rc)
+    raw, res, pos = bytes(out), [], 0
+    for s in range(n):
+        res.append((st[s], raw[pos:pos + ln[s]], bool(mv[s])))
+        pos += ln[s]
+    return res, bad.value
 
 
 # ---- baseline Huffman decode kernels (lep_huff.cu, lep_huffpar.cu)

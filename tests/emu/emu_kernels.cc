@@ -177,7 +177,7 @@ struct EncArgs {
     int stage;                       // 0 count, 1 offsets, 2 symbolise (kernel A), 3 range coder (kernel B)
     const ImageDesc* images; SegDesc* segs; int nseg; const int* order; int* counter;
     uint16_t* models; uint8_t* rows; size_t row_stride; uint16_t* tokens; unsigned long long* total;
-    unsigned long long* ck; uint32_t* digits;
+    unsigned long long* ck; uint32_t* digits; uint8_t* ovf;
 };
 
 void enc_body(void* p) {
@@ -188,9 +188,56 @@ void enc_body(void* p) {
     else if (a.stage == 3) lep_rangecode_kernel(a.segs, a.nseg, a.order, a.tokens);
     else if (a.stage == 5) lep_rangepass_kernel<true>(a.segs, a.nseg, a.order, a.tokens, a.ck);
     else if (a.stage == 4) lep_rangepass_kernel<false>(a.segs, a.nseg, a.order, a.tokens, a.ck);
-    else if (a.stage == 6) lep_digit_offsets_kernel(a.segs, a.nseg, a.total);
+    else if (a.stage == 6) lep_digit_offsets_kernel(a.segs, a.nseg, a.total, a.total + 1);
     else if (a.stage == 7) lep_rangepiece_kernel(a.segs, a.nseg, a.tokens, a.ck, a.digits);
-    else lep_rangenorm_kernel(a.segs, a.nseg, a.order, a.digits);
+    else lep_rangenorm_kernel(a.segs, a.nseg, a.order, a.digits, a.ovf);
+}
+
+// Kernel B after kernel A, with the launch shapes and the host steps of lepb200_encode_launch_rangecode /
+// lepb200_encode_fetch (lep_capi.cu): kernel 0 / 2 = the parallel range coder (async / register token feed): range pass,
+// digit offsets (+ overflow slots: `ovf` receives the overflow arena), pieces, carries; kernel 1 = the serial coder, then
+// rerun_overflowed_serial for the segments whose stream outgrew the slot.  `total_tokens` = size of the token arena.
+void run_range_coder(int kernel, EncArgs& a, unsigned long long total_tokens, std::vector<uint8_t>& ovf) {
+    const int nseg = a.nseg;
+    std::vector<unsigned long long> ck;
+    std::vector<uint32_t> digits;
+    if (kernel == 0 || kernel == 2) {
+        ck.assign(((size_t)total_tokens >> 10) + 2 * (size_t)nseg + 8, 0);
+        a.ck = ck.data();
+        a.stage = kernel == 0 ? 5 : 4; emu::launch((unsigned)((nseg + RCT_THREADS - 1) / RCT_THREADS), RCT_THREADS, enc_body, &a);
+        unsigned long long totals[2] = {0, 0};
+        a.total = totals;
+        a.stage = 6; emu::launch(1, 1024, enc_body, &a);
+        digits.assign((size_t)totals[0] + 64, 0);
+        ovf.assign((size_t)totals[1] + 256, 0xC3);                 // + 256 canary bytes (emu_range_code)
+        a.digits = digits.data();
+        a.ovf = ovf.data();
+        a.stage = 7;
+        for (int y = 0; y < nseg; ++y) { emu::g_block_idx.y = (unsigned)y; emu::launch(8, RCP_THREADS, enc_body, &a); }      // grid (8, nseg)
+        emu::g_block_idx.y = 0;
+        a.stage = 8; emu::launch((unsigned)((nseg + RCN_WARPS - 1) / RCN_WARPS), RCN_WARPS * 32, enc_body, &a);
+        return;
+    }
+    a.stage = 3; emu::launch((unsigned)((nseg + RC_THREADS - 1) / RC_THREADS), RC_THREADS, enc_body, &a);
+    std::vector<int> redo;                       // rerun_overflowed_serial
+    size_t total = 0;
+    auto bound = [](uint32_t ntok) { return align_up((7ull * ((unsigned long long)ntok + 33) + 8) / 8 + 2, 256); };
+    for (int s = 0; s < nseg; ++s)
+        if (a.segs[s].status == ST_OUT_OVERFLOW && a.segs[s].ntok <= a.segs[s].tok_cap) { redo.push_back(s); total += bound(a.segs[s].ntok); }
+    if (redo.empty()) return;
+    ovf.assign(total + 256, 0xC3);
+    size_t off = 0;
+    for (int s : redo) {
+        SegDesc& sd = a.segs[s];
+        sd.stream = (unsigned long long)(uintptr_t)(ovf.data() + off);
+        sd.cap = (uint32_t)bound(sd.ntok);
+        sd.status = ST_OK; sd.len = 0;
+        off += sd.cap;
+    }
+    const int* order = a.order;
+    a.order = redo.data(); a.nseg = (int)redo.size();
+    a.stage = 3; emu::launch((unsigned)((redo.size() + RC_THREADS - 1) / RC_THREADS), RC_THREADS, enc_body, &a);
+    a.order = order; a.nseg = nseg;
 }
 
 }  // namespace
@@ -199,8 +246,10 @@ void enc_body(void* p) {
 // (range coder), with the launch shapes of lep_capi.cu.  `out` must hold sum(nseg) entries; the bytes of every stream are
 // copied into `arena` (capacity arena_cap) back to back and out[i].data points there.  grid_cap > 0 limits kernel A's
 // CTAs (persistent warps then take several segments each).  kernel: 0 = parallel range coder, 1 = serial range coder,
-// 2 = parallel range coder whose range pass feeds tokens through registers (LEPB200_RC_FEED=0).
-extern "C" int emu_encode_images(int kernel, int grid_cap, const lepb200_image* images, int nimages, lepb200_stream* out, uint8_t* arena, size_t arena_cap) {
+// 2 = parallel range coder whose range pass feeds tokens through registers (LEPB200_RC_FEED=0).  tok_caps (optional,
+// sum(nseg) entries) receives the token bound of every segment (the count pre-pass's, or the caller's seg_token_bound).
+extern "C" int emu_encode_images(int kernel, int grid_cap, const lepb200_image* images, int nimages, lepb200_stream* out, uint8_t* arena, size_t arena_cap,
+                                 uint32_t* tok_caps) {
     if (nimages <= 0 || !images || !out || !arena) return LEPB200_ERR_INVALID;
     std::vector<ImageDesc> descs(nimages);
     std::vector<SegDesc> segs;
@@ -277,24 +326,10 @@ extern "C" int emu_encode_images(int kernel, int grid_cap, const lepb200_image* 
         for (int s = 0; f && s < nseg; ++s) { const uint32_t nt = segs[s].ntok; fwrite(&nt, 4, 1, f); fwrite(tokens.data() + segs[s].tokens, 2, nt, f); }
         if (f) fclose(f);
     }
-    std::vector<unsigned long long> ck;
-    std::vector<uint32_t> digits;
-    if (kernel == 0 || kernel == 2) {   // parallel range coder: range-only pass, digit layout, pieces, carries (lep_capi.cu: rc_mode 1; 2 = register-ring token feed)
-        ck.assign(((size_t)total_tokens >> 10) + 2 * (size_t)nseg + 8, 0);
-        a.ck = ck.data();
-        a.stage = kernel == 0 ? 5 : 4; emu::launch((unsigned)((nseg + RCT_THREADS - 1) / RCT_THREADS), RCT_THREADS, enc_body, &a);
-        unsigned long long total_digits = 0;
-        a.total = &total_digits;
-        a.stage = 6; emu::launch(1, 1024, enc_body, &a);
-        digits.assign((size_t)total_digits + 64, 0);
-        a.digits = digits.data();
-        a.stage = 7;
-        for (int y = 0; y < nseg; ++y) { emu::g_block_idx.y = (unsigned)y; emu::launch(8, RCP_THREADS, enc_body, &a); }      // grid (8, nseg)
-        emu::g_block_idx.y = 0;
-        a.stage = 8; emu::launch((unsigned)((nseg + RCN_WARPS - 1) / RCN_WARPS), RCN_WARPS * 32, enc_body, &a);
-    } else {                  // kernel 1: the serial range coder (rc_mode 0)
-        a.stage = 3; emu::launch((unsigned)((nseg + RC_THREADS - 1) / RC_THREADS), RC_THREADS, enc_body, &a);
-    }
+    // parallel range coder (lep_capi.cu: rc_mode 1; kernel 2 = register-ring token feed) or the serial one (kernel 1, rc_mode 0)
+    std::vector<uint8_t> ovf;
+    run_range_coder(kernel, a, total_tokens, ovf);
+    if (tok_caps) for (int s = 0; s < nseg; ++s) tok_caps[s] = segs[s].tok_cap;
     size_t used = 0;
     for (int s = 0; s < nseg; ++s) {
         const size_t n = segs[s].status == 0 ? segs[s].len : 0;
@@ -310,6 +345,74 @@ extern "C" int emu_encode_images(int kernel, int grid_cap, const lepb200_image* 
     return 0;
 }
 
+
+// ---- kernel B alone on given token streams.  Segment s has ntok[s] tokens (prob | bit << 8, all segments back to back in
+// `tokens`) and a stream slot of caps[s] bytes.  The tokens are laid out like lep_token_offsets_kernel lays them out (tok_cap
+// = ntok rounded up to 64 tokens after 64 of slack, so piece checkpoints sit at (tokens >> 10) + 2 * segment), the
+// segments run in the order of lepb200_encode (longest first), and kernel B runs as run_range_coder runs it, overflow
+// handling included.  256 canary bytes follow every slot and the overflow arena.  reverse = 1 runs every launch's
+// CTAs and threads in reverse order (emu::g_reverse).  Outputs per segment: status, len, moved (1 = the stream ended up in the
+// overflow arena), its bytes back to back in `out` (out_cap bytes); *canary_bad = canary bytes that changed.
+extern "C" int emu_range_code(int kernel, int reverse, int nseg, const uint16_t* tokens, const uint32_t* ntok, const uint32_t* caps,
+                              int32_t* status_out, uint32_t* len_out, uint8_t* moved_out, uint8_t* out, size_t out_cap, uint64_t* canary_bad) {
+    if (nseg <= 0 || !tokens || !ntok || !caps || !out || !canary_bad || (kernel != 0 && kernel != 1 && kernel != 2)) return LEPB200_ERR_INVALID;
+    constexpr size_t CANARY = 256;
+    constexpr uint8_t CANARY_BYTE = 0xC3;
+    std::vector<SegDesc> segs(nseg);
+    std::vector<size_t> slot(nseg);
+    unsigned long long total_tokens = 0;
+    size_t stream_total = 0, src = 0;
+    for (int s = 0; s < nseg; ++s) {
+        SegDesc& sd = segs[s];
+        memset(&sd, 0, sizeof(sd));
+        sd.ntok = ntok[s];
+        sd.tok_cap = (uint32_t)(((unsigned long long)ntok[s] + 64 + 63) & ~63ull);
+        sd.tokens = total_tokens;
+        total_tokens += sd.tok_cap;
+        sd.cap = caps[s];
+        slot[s] = stream_total;
+        stream_total += align_up((size_t)caps[s] + CANARY, 256);
+    }
+    std::vector<uint16_t> tok((size_t)total_tokens + 128, 0);
+    for (int s = 0; s < nseg; ++s) { memcpy(tok.data() + segs[s].tokens, tokens + src, (size_t)ntok[s] * 2); src += ntok[s]; }
+    std::vector<uint8_t> streams(stream_total + 256, CANARY_BYTE);
+    uint8_t* sbase = reinterpret_cast<uint8_t*>(align_up((size_t)(uintptr_t)streams.data(), 256));
+    for (int s = 0; s < nseg; ++s) segs[s].stream = (unsigned long long)(uintptr_t)(sbase + slot[s]);
+    std::vector<int> order(nseg);
+    for (int i = 0; i < nseg; ++i) order[i] = i;
+    std::stable_sort(order.begin(), order.end(), [&](int a, int b) { return ntok[a] > ntok[b]; });
+    EncArgs a;
+    memset(&a, 0, sizeof(a));
+    a.segs = segs.data(); a.nseg = nseg; a.order = order.data(); a.tokens = tok.data();
+    std::vector<uint8_t> ovf;
+    emu::g_reverse = reverse != 0;
+    run_range_coder(kernel, a, total_tokens, ovf);
+    emu::g_reverse = false;
+    uint64_t bad = 0;
+    for (int s = 0; s < nseg; ++s) {
+        const uint8_t* p = sbase + slot[s];
+        for (size_t k = caps[s]; k < align_up((size_t)caps[s] + CANARY, 256); ++k) bad += p[k] != CANARY_BYTE;
+    }
+    size_t used = 0;
+    for (int s = 0; s < nseg; ++s) {
+        const uint8_t* p = reinterpret_cast<const uint8_t*>(segs[s].stream);
+        const bool moved = p < sbase || p >= sbase + stream_total;
+        if (moved) {              // an overflow slot: the bytes of the arena behind the stream are the next slot's or the canary
+            const size_t end = (size_t)(p - ovf.data()) + segs[s].cap;
+            if (end > ovf.size()) return LEPB200_ERR_INVALID;
+        }
+        const size_t n = segs[s].status == 0 ? segs[s].len : 0;
+        if (used + n > out_cap) return LEPB200_ERR_NOMEM;
+        memcpy(out + used, p, n);
+        used += n;
+        status_out[s] = segs[s].status;
+        len_out[s] = n;
+        moved_out[s] = moved ? 1 : 0;
+    }
+    if (!ovf.empty()) for (size_t k = ovf.size() - 256; k < ovf.size(); ++k) bad += ovf[k] != CANARY_BYTE;
+    *canary_bad = bad;
+    return 0;
+}
 
 // ---- baseline Huffman decode: lep_huffdecode_kernel alone (mode 0) or the sub-sequence kernels of lep_huffpar.cu followed
 // by it (mode 1), with the job set-up and the iteration loop of lepb200_huffman_decode_to_device (lep_capi.cu).

@@ -46,6 +46,25 @@ def load_extreme_lep(name):
     return lepfmt.parse_container(read_golden("extremes/" + name))
 
 
+# white-noise JPEGs whose every thread-segment needs more stream than its initial slot (tests/golden/make_dense.py)
+DENSE = json.load(open(os.path.join(GOLDEN, "dense.json")))
+
+
+def dense_jpegs():
+    return sorted(n for n in DENSE if n.endswith(".jpg"))
+
+
+def dense_leps():
+    """(name of the .lep, name of its source JPEG) for every reference-written .lep of the dense corpus."""
+    out = [(n[:-4] + ".lep", n) for n in dense_jpegs()]
+    out += [(n, e["source"]) for n, e in DENSE.items() if n.endswith(".lep")]
+    return sorted(out)
+
+
+def load_dense_lep(name):
+    return lepfmt.parse_container(read_golden("dense/" + name))
+
+
 def geometry_of(lf):
     f = lf.frame
     tbcv, tbc = lepfmt.truncation(lf)
@@ -87,13 +106,16 @@ def coef_image_from_lep(lf, planes):
 
 
 def random_coef_image(rng, ncmp=3, mcuh=5, mcuv=4, sf=((2, 2), (1, 1), (1, 1)), density=0.25, amp=60, nseg=1,
-                      qscale=1, q16=False, max_cat=0, dc_max=1000):
+                      qscale=1, q16=False, max_cat=0, dc_max=1000, noise=None):
     """Synthetic coefficient planes with JPEG-like statistics (sparse, decaying with frequency).
 
     The knobs that leave photo statistics behind: q16 draws every quantiser uniformly from the 16-bit range 1..65535;
     max_cat > 0 draws the magnitude category of every kept coefficient uniformly from 0..max_cat (then uniformly inside the
     category) instead of the geometric magnitudes; dc_max bounds the DC random walk (up to 2047; values beyond 1024 make
-    the reference refuse the segment with status 6)."""
+    the reference refuse the segment with status 6).  noise = "gauss" or "uniform" replaces the AC coefficients by iid
+    noise at every position, N(0, amp) rounded or uniform over -amp..amp (clipped to +-1023), and sets every quantiser
+    to 1 but the DC one (8, so that the DC predictions stay codable): white noise as a quality-100 encoder sees it, the
+    densest streams a JPEG can give the coder."""
     from lepton_b200 import CoefImage
     bch = [mcuh * sf[c][0] for c in range(ncmp)]
     bcv = [mcuv * sf[c][1] for c in range(ncmp)]
@@ -112,12 +134,20 @@ def random_coef_image(rng, ncmp=3, mcuh=5, mcuv=4, sf=((2, 2), (1, 1), (1, 1)), 
         sign = rng.integers(0, 2, size=(n, 64)) * 2 - 1
         p = (mag * keep * sign).astype(np.int16)
         p = np.clip(p, -2047, 2047).astype(np.int16)
+        if noise == "gauss":
+            p = np.clip(np.rint(rng.normal(0, amp, size=(n, 64))), -1023, 1023).astype(np.int16)
+        elif noise == "uniform":
+            p = rng.integers(-amp, amp + 1, size=(n, 64)).clip(-1023, 1023).astype(np.int16)
+        else:
+            assert noise is None, noise
         if dc_max > 1000:
             p[:, 49] = rng.integers(-dc_max, dc_max + 1, size=n)
         else:
             p[:, 49] = np.clip(np.cumsum(rng.integers(-20, 21, size=n)), -dc_max, dc_max)  # smooth DC
         planes.append(np.ascontiguousarray(p))
-    if q16:
+    if noise:
+        q = [[8] + [1] * 63 for _ in range(ncmp)]
+    elif q16:
         q = [[int(v) for v in rng.integers(1, 65536, size=64)] for _ in range(ncmp)]
     else:
         q = [[max(1, min(255, int((3 + i // 4) * qscale))) for i in range(64)] for _ in range(ncmp)]
