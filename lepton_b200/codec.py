@@ -417,6 +417,8 @@ class HostJpeg:
                          bcv=[im.bcv[c] for c in range(im.ncmp)],
                          qtables_zigzag=[[im.qtable_zigzag[c][i] for i in range(64)] for c in range(im.ncmp)],
                          planes=planes, luma_y_start=[im.luma_y_start[s] for s in range(im.nseg)],
+                         trunc_bcv=[im.trunc_bcv[c] for c in range(im.ncmp)],
+                         trunc_bc=[im.trunc_bc[c] for c in range(im.ncmp)],
                          jpeg_bytes=len(self._data), _keep=[self])
 
     def write_lep(self, streams: Sequence[bytes]) -> bytes:
@@ -469,7 +471,9 @@ class HostLep:
         return CoefImage(ncmp=im.ncmp, mcuv=im.mcuv, bch=[im.bch[c] for c in range(im.ncmp)],
                          bcv=[im.bcv[c] for c in range(im.ncmp)],
                          qtables_zigzag=[[im.qtable_zigzag[c][i] for i in range(64)] for c in range(im.ncmp)],
-                         planes=planes, luma_y_start=[im.luma_y_start[s] for s in range(im.nseg)])
+                         planes=planes, luma_y_start=[im.luma_y_start[s] for s in range(im.nseg)],
+                         trunc_bcv=[im.trunc_bcv[c] for c in range(im.ncmp)],
+                         trunc_bc=[im.trunc_bc[c] for c in range(im.ncmp)])
 
     def scan_layout(self):
         """(offset, length) of the entropy-coded scan in the original JPEG, (0, 0) if the host has to re-encode it."""

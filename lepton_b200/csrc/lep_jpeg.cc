@@ -323,6 +323,20 @@ inline int decode_symbol_value(BitReader& br, const HuffTable& t, int size_mask,
     }
     const int s = sym & size_mask;
     int v = 0;
+    const uint64_t p = br.bitpos + (uint64_t)len, end = (uint64_t)br.n * 8, tail = (uint64_t)(br.n & ~(size_t)7) * 8;
+    if (s && (br.n & 7) && p < tail && p + (uint64_t)s > end) {
+        // Magnitude bits that run past the end of truncated data across the start of its last, partial 8-byte word.
+        // The reference's abitreader loads the data 8 bytes at a time; a read that needs more bits than that last
+        // load holds takes them right-aligned (bitops.hh:294-301), so the missing bits sit between the two parts, not
+        // at the end, and eof is only set by the next read (the reader is left at the end, not yet at eof).
+        const int k = (int)(tail - p);
+        uint32_t lastw = 0;
+        for (size_t i = br.n & ~(size_t)7; i < br.n; ++i) lastw = (lastw << 8) | br.d[i];
+        const int nb = (int)((((win << len) >> (64 - k)) << (s - k)) | lastw) & ((1 << s) - 1);
+        *value = nb >= (1 << (s - 1)) ? nb : nb + 1 - (1 << s);
+        br.bitpos = end;
+        return sym;
+    }
     if (s) {
         const int nb = (int)((win << len) >> (64 - s));
         v = nb >= (1 << (s - 1)) ? nb : nb + 1 - (1 << s);

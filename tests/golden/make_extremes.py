@@ -42,7 +42,12 @@ from jpegwriter import AC_SYMBOLS, DC_SYMBOLS, HuffTable, fit_lengths, geometry,
 LEPTON = os.path.join(ROOT, "oracle", "_ref", "lepton")
 OUTDIR = os.path.join(HERE, "extremes")
 OUT = os.path.join(HERE, "extremes.json")
-EXIT_CODES = {"COEFFICIENT_OUT_OF_RANGE": 6}
+# ExitCode values of the reference (src/vp8/util/memory.hh); a run that prints one of these names failed with it, even
+# when the process itself exits with 0
+EXIT_CODES = {"ASSERTION_FAILURE": 1, "CODING_ERROR": 2, "SHORT_READ": 3, "UNSUPPORTED_4_COLORS": 4, "THREAD_PROTOCOL_ERROR": 5,
+              "COEFFICIENT_OUT_OF_RANGE": 6, "STREAM_INCONSISTENT": 7, "PROGRESSIVE_UNSUPPORTED": 8,
+              "SAMPLING_BEYOND_TWO_UNSUPPORTED": 10, "SAMPLING_BEYOND_FOUR_UNSUPPORTED": 11, "THREADING_PARTIAL_MCU": 12,
+              "ONLY_GARBAGE_NO_JPEG": 14, "UNSUPPORTED_JPEG": 42, "UNSUPPORTED_JPEG_WITH_ZERO_IDCT_0": 43}
 RASTER_OF_ZZ = [0, 1, 8, 16, 9, 2, 3, 10, 17, 24, 32, 25, 18, 11, 4, 5, 12, 19, 26, 33, 40, 48, 41, 34, 27, 20, 13, 6, 7, 14,
                 21, 28, 35, 42, 49, 56, 57, 50, 43, 36, 29, 22, 15, 23, 30, 37, 44, 51, 58, 59, 52, 45, 38, 31, 39, 46, 53, 60,
                 61, 54, 47, 55, 62, 63]

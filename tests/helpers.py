@@ -65,6 +65,49 @@ def load_dense_lep(name):
     return lepfmt.parse_container(read_golden("dense/" + name))
 
 
+# small baseline JPEGs cut at every byte of their scan and what the reference CLI made of every cut
+# (tests/golden/make_truncated.py)
+TRUNCATED = json.load(open(os.path.join(GOLDEN, "truncated.json")))
+TRUNC_THREADS = {"t1": 1, "t4": 4, "t8": 8}          # record name -> -minencodethreads
+
+
+def truncated_sources():
+    return sorted(TRUNCATED["sources"])
+
+
+# the status the library reports for each code of truncated.json (a 5 of the reference's threads comes with a 6)
+TRUNC_STATUS = {"r": 0, "n": 0, "c": 6, "t": 6, "u": 42}
+
+
+def truncated_cuts(name, flag="t1"):
+    """(cut, code of truncated.json) for every cut of a source; the cut's bytes are truncated_source(name)[:cut]."""
+    first = TRUNCATED["sources"][name]["first_cut"]
+    return [(first + i, k) for i, k in enumerate(TRUNCATED["runs"][name][flag]["codes"])]
+
+
+def lep_chain(leps):
+    """md5 over the md5s of .lep files in cut order, as truncated.json's lep_chain of a run."""
+    return hashlib.md5("".join(hashlib.md5(b).hexdigest() for b in leps).encode()).hexdigest()
+
+
+def truncated_source(name):
+    return read_golden(TRUNCATED["sources"][name]["path"])
+
+
+def truncated_leps():
+    """Names of the committed reference .lep files of cuts, in a fixed order."""
+    return sorted(TRUNCATED["leps"])
+
+
+def load_truncated_lep(name):
+    return lepfmt.parse_container(read_golden("truncated/" + name))
+
+
+def truncated_cut_of(lep_name):
+    e = TRUNCATED["leps"][lep_name]
+    return truncated_source(e["source"])[:e["cut"]]
+
+
 def geometry_of(lf):
     f = lf.frame
     tbcv, tbc = lepfmt.truncation(lf)
@@ -105,8 +148,42 @@ def coef_image_from_lep(lf, planes):
                      jpeg_bytes=lf.jpeg_size)
 
 
+def truncation_bounds(bch, bcv, mcuv, max_dpos):
+    """(trunc_bcv, trunc_bc) of a scan that ended after block max_dpos[c] of every component, by the JPEG front end's
+    rule (lep_jpeg.cc, after the scan loop): the coded blocks are max_dpos + 1, the coded rows those blocks touch rounded
+    up to whole MCU rows of the component -- so the last of those rows can lie wholly past the coded blocks."""
+    tbcv, tbc = [], []
+    for c in range(len(bch)):
+        n = max_dpos[c] + 1
+        vs = min(-(-n // bch[c]), bcv[c])
+        ratio = bcv[c] // mcuv
+        while vs % ratio and vs + 1 <= bcv[c]:
+            vs += 1
+        tbcv.append(vs)
+        tbc.append(n)
+    return tbcv, tbc
+
+
+def random_cut(rng, ncmp, mcuh, mcuv, sf):
+    """The last block of every component that a scan cut at a random block (in scan order) decoded: interleaved MCUs for
+    colour, the plain raster for one component."""
+    bch = [mcuh * sf[c][0] for c in range(ncmp)]
+    order = []
+    for mcu in range(mcuh * mcuv):
+        my, mx = divmod(mcu, mcuh)
+        for c in range(ncmp):
+            for sy in range(sf[c][1]):
+                for sx in range(sf[c][0]):
+                    order.append((c, (my * sf[c][1] + sy) * bch[c] + mx * sf[c][0] + sx))
+    g = int(rng.integers(0, len(order)))
+    max_dpos = [0] * ncmp
+    for c, d in order[:g + 1]:
+        max_dpos[c] = max(max_dpos[c], d)
+    return max_dpos
+
+
 def random_coef_image(rng, ncmp=3, mcuh=5, mcuv=4, sf=((2, 2), (1, 1), (1, 1)), density=0.25, amp=60, nseg=1,
-                      qscale=1, q16=False, max_cat=0, dc_max=1000, noise=None):
+                      qscale=1, q16=False, max_cat=0, dc_max=1000, noise=None, trunc=False):
     """Synthetic coefficient planes with JPEG-like statistics (sparse, decaying with frequency).
 
     The knobs that leave photo statistics behind: q16 draws every quantiser uniformly from the 16-bit range 1..65535;
@@ -115,7 +192,11 @@ def random_coef_image(rng, ncmp=3, mcuh=5, mcuv=4, sf=((2, 2), (1, 1), (1, 1)), 
     the reference refuse the segment with status 6).  noise = "gauss" or "uniform" replaces the AC coefficients by iid
     noise at every position, N(0, amp) rounded or uniform over -amp..amp (clipped to +-1023), and sets every quantiser
     to 1 but the DC one (8, so that the DC predictions stay codable): white noise as a quality-100 encoder sees it, the
-    densest streams a JPEG can give the coder."""
+    densest streams a JPEG can give the coder.  trunc=True makes the image a truncated scan: a cut block drawn in scan
+    order (random_cut) gives trunc_bcv / trunc_bc by the front end's rule (truncation_bounds); trunc="any" draws the last
+    block of every component on its own, as files whose components sit in separate scans can end (a chroma scan before
+    the luma scan leaves chroma rows past the last luma row).  The planes keep their
+    random data past the bounds, so a kernel that codes a block it should skip changes the stream."""
     from lepton_b200 import CoefImage
     bch = [mcuh * sf[c][0] for c in range(ncmp)]
     bcv = [mcuv * sf[c][1] for c in range(ncmp)]
@@ -153,7 +234,27 @@ def random_coef_image(rng, ncmp=3, mcuh=5, mcuv=4, sf=((2, 2), (1, 1), (1, 1)), 
         q = [[max(1, min(255, int((3 + i // 4) * qscale))) for i in range(64)] for _ in range(ncmp)]
     v0 = bcv[0] // mcuv
     starts = sorted({(k * mcuv // nseg) * v0 for k in range(nseg)})
-    return CoefImage(ncmp=ncmp, mcuv=mcuv, bch=bch, bcv=bcv, qtables_zigzag=q, planes=planes, luma_y_start=starts)
+    tbcv = tbc = None
+    if trunc == "any":
+        tbcv, tbc = truncation_bounds(bch, bcv, mcuv, [int(rng.integers(0, bch[c] * bcv[c])) for c in range(ncmp)])
+    elif trunc:
+        tbcv, tbc = truncation_bounds(bch, bcv, mcuv, random_cut(rng, ncmp, mcuh, mcuv, sf))
+    return CoefImage(ncmp=ncmp, mcuv=mcuv, bch=bch, bcv=bcv, qtables_zigzag=q, planes=planes, luma_y_start=starts,
+                     trunc_bcv=tbcv, trunc_bc=tbc)
+
+
+def oracle_decode_image(img, streams):
+    """Planes the ORACLE decodes from per-segment streams of a CoefImage's geometry (zero where nothing is coded)."""
+    g = oracle.make_geometry(img.ncmp, list(img.bch), list(img.bcv), img.mcuv, img.qtables_zigzag,
+                             list(img.trunc_bcv) if img.trunc_bcv is not None else None,
+                             list(img.trunc_bc) if img.trunc_bc is not None else None)
+    planes = [np.zeros_like(p) for p in img.planes]
+    starts = list(img.luma_y_start)
+    for i, y0 in enumerate(starts):
+        last = i == len(starts) - 1
+        rc, _ = oracle.decode_segment(g, planes, y0, img.bcv[0] if last else starts[i + 1], last, streams[i])
+        assert rc == 0, (i, rc)
+    return planes
 
 
 def mixed_corpus_jpegs():
