@@ -41,7 +41,7 @@ def build(force=False, verbose=False, variant=None):
 def _build(verbose, cli):
     cu = [os.path.join(SRC, "lep_capi.cu")]
     cc = sorted(os.path.join(SRC, f) for f in os.listdir(SRC) if f.endswith(".cc") and f != "lepton_cli.cc")
-    defs = ["-D%s=%s" % (k, os.environ[k]) for k in ("LEPB200_ENC_MINBLOCKS", "LEPB200_DEC_MINBLOCKS", "LEPB200_HUFF_MINBLOCKS", "LEPB200_STREAM_HINTS", "LEPB200_G2_PREFETCH", "LEPB200_G2_PF_DIST") if k in os.environ]
+    defs = ["-D%s=%s" % (k, os.environ[k]) for k in ("LEPB200_ENC_MINBLOCKS", "LEPB200_DEC_MINBLOCKS", "LEPB200_HUFF_MINBLOCKS", "LEPB200_STREAM_HINTS") if k in os.environ]
     cmd = [NVCC, "-gencode", "arch=compute_90a,code=sm_90a", "-lineinfo", "-O3", "-std=c++17", "-shared"] + defs + [
            "-Xcompiler", "-fPIC,-O3,-pthread", "-o", OUT] + cu + cc + ["-lz", "-lpthread", "-ldl"]
     if verbose:

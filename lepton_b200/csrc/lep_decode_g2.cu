@@ -9,6 +9,7 @@
 //     contexts (Lakhani prior -> bsr, sign class, threshold context), per-component table bases by remaining count;
 //   * end-of-block positions (eob_x / eob_y) are found by the lanes after the 7x7 loop instead of per decision, the
 //     residual / threshold table addresses are formed only when a coefficient turns out to need them;
+//   * the count trees are read as whole rows before their first bit, so no bit of a count waits for a load;
 //   * the stream window is topped up from a word fetched one refill ahead.
 //
 // Same job descriptors, model layout, work queue and results as lep_decode_group.cu.
@@ -96,23 +97,35 @@ __device__ __forceinline__ uint32_t g2_get(G2Bool& r, uint16_t* model, const uin
 #define G2_EMU_BARRIER()
 #endif
 
-// Model lines a group will need a few decisions from now are requested ahead of time (the batch keeps ~800 MB of hot
-// model lines alive, far more than the L2 holds, so a demand load is a DRAM round trip on the serial chain).
-// G2_PF_DIST: how many coefficients ahead of the one being decoded.
-#ifndef LEPB200_G2_PREFETCH
-#define LEPB200_G2_PREFETCH 0
-#endif
-#if LEPB200_G2_PREFETCH == 1 && !defined(LEPB200_EMU)
-__device__ __forceinline__ void g2_prefetch(const uint16_t* p) { asm volatile("prefetch.global.L1 [%0];" ::"l"(p)); }
-#elif LEPB200_G2_PREFETCH == 2 && !defined(LEPB200_EMU)
-__device__ __forceinline__ void g2_prefetch(const uint16_t* p) { asm volatile("prefetch.global.L2 [%0];" ::"l"(p)); }
-#else
-__device__ __forceinline__ void g2_prefetch(const uint16_t*) {}
-#endif
-#ifndef LEPB200_G2_PF_DIST
-#define LEPB200_G2_PF_DIST 3
-#endif
-constexpr int G2_PF_DIST = LEPB200_G2_PF_DIST;
+// Branch words of the fixed-length count trees are read as whole rows (a tree level's candidates are contiguous), so
+// that no bit of a count waits for a load the previous bit chose: halfword i of 8 packed in a uint4, of 4 in a uint2.
+__device__ __forceinline__ uint32_t g2_half8(uint4 v, uint32_t i) {
+    const uint32_t u = (i & 4u) ? ((i & 2u) ? v.w : v.z) : ((i & 2u) ? v.y : v.x);
+    return (u >> ((i & 1u) << 4)) & 0xffffu;
+}
+__device__ __forceinline__ uint32_t g2_half4(uint2 v, uint32_t i) {
+    return (((i & 2u) ? v.y : v.x) >> ((i & 1u) << 4)) & 0xffffu;
+}
+// the 7x7 count tree (m_nz7): rows 5..2 hold 1, 2, 4, 8 words at the row start and do not depend on a bit of the count,
+// so they are requested together, as early as the tree's base is known
+struct G2NzTop { uint32_t r5, r4; uint2 r3; uint4 r2; };
+__device__ __forceinline__ G2NzTop g2_nz_top(const uint16_t* t) {
+    G2NzTop v;
+    v.r5 = t[5 << 5];
+    v.r4 = *reinterpret_cast<const uint32_t*>(t + (4 << 5));
+    v.r3 = *reinterpret_cast<const uint2*>(t + (3 << 5));
+    v.r2 = *reinterpret_cast<const uint4*>(t + (2 << 5));
+    return v;
+}
+// an edge count tree (m_nze): rows 2, 1, 0 of 1, 2, 4 words, 24 bytes in all
+struct G2EdgeTree { uint32_t r2, r1; uint2 r0; };
+__device__ __forceinline__ G2EdgeTree g2_edge_tree(const uint16_t* t) {
+    G2EdgeTree v;
+    v.r2 = t[2 << 2];
+    v.r1 = *reinterpret_cast<const uint32_t*>(t + (1 << 2));
+    v.r0 = *reinterpret_cast<const uint2*>(t);
+    return v;
+}
 
 enum : int { G2_EXP = 0, G2_SIGN = 1, G2_THR = 2, G2_RES = 3 };
 
@@ -216,6 +229,11 @@ lep_decode_g2_kernel(const ImageDesc* __restrict__ images, SegDesc* __restrict__
     const int32_t* icx = nullptr;
     const int32_t* icy = nullptr;
     const uint8_t* mthr = nullptr;
+    // ---- the 7x7 count tree of the block to come: base and top rows, requested at the end of the previous block of the
+    //      row when it has one (in flight during phases (1) and (1b)), else in (1b)
+    uint32_t cnt_addr = 0;
+    G2NzTop nzt = {};
+    bool cnt_ready = false;
 
     for (;;) {
         // ---- (0a) a free group takes the next segment of the queue
@@ -305,7 +323,6 @@ lep_decode_g2_kernel(const ImageDesc* __restrict__ images, SegDesc* __restrict__
         }
         __syncwarp();
         // ---- (1b) exponent offsets of the 49 inner positions: compute_aavrg (model.hh:895-924) -> bit length -> (zz*12+bsr)<<4
-        uint32_t cnt_addr = 0;
         if (alive) {
             for (int zz = sub; zz < 49; zz += G) {
                 const int coord = s_a2r[zz];
@@ -319,34 +336,42 @@ lep_decode_g2_kernel(const ImageDesc* __restrict__ images, SegDesc* __restrict__
                 }
                 eoff[zz] = (uint16_t)((zz * 12 + bitlen(min(pr, 1023u))) << 4);
             }
-            const int nz_above = has_above ? (int)rnz[x] : 0;
-            int ctx = 0;
-            if (has_above && !has_left) ctx = (nz_above + 1) / 2;
-            else if (has_left && !has_above) ctx = (nz_left + 1) / 2;
-            else if (has_left && has_above) ctx = (nz_above + nz_left + 2) / 4;
-            cnt_addr = m_nz7(ci, s_nzbin[ctx], 0, 0);
+            if (!cnt_ready) {
+                const int nz_above = has_above ? (int)rnz[x] : 0;
+                int ctx = 0;
+                if (has_above && !has_left) ctx = (nz_above + 1) / 2;
+                else if (has_left && !has_above) ctx = (nz_left + 1) / 2;
+                else if (has_left && has_above) ctx = (nz_above + nz_left + 2) / 4;
+                cnt_addr = m_nz7(ci, s_nzbin[ctx], 0, 0);
+                nzt = g2_nz_top(model + cnt_addr);
+            }
         }
+        cnt_ready = false;
         __syncwarp();
 
-        // ---- (2a) the 7x7 non-zero count: six decisions, every live group in step (decoder.cc:175-184).  The branch word of
-        //      the next level is requested as soon as this level's bit is known, before the write-back.
+        // ---- (2a) the 7x7 non-zero count: six decisions, every live group in step (decoder.cc:175-184).  Level idx of the
+        //      tree is the row cnt_addr + idx * 32, indexed by the bits above it.  Rows 5..2 are in registers already; the
+        //      8 words of row 1 that the first bit leaves possible, and of row 0 after the second bit, are requested three
+        //      decisions before they are used.  No word of the tree is read twice, so nothing needs forwarding.
         {
-            uint32_t prefix = 0, a = cnt_addr + (5u << 5);
-            uint32_t mw = alive ? model[a] : 0u;
-            G2_EMU_BARRIER();
-#pragma unroll 1
+            uint4 r1 = make_uint4(0u, 0u, 0u, 0u), r0 = r1;
+            uint32_t prefix = 0;
+#pragma unroll
             for (int idx = 5; idx >= 0; --idx) {
+                const uint32_t mw = idx == 5 ? nzt.r5 : idx == 4 ? (nzt.r4 >> (prefix << 4)) & 0xffffu
+                                  : idx == 3 ? g2_half4(nzt.r3, prefix) : idx == 2 ? g2_half8(nzt.r2, prefix)
+                                  : idx == 1 ? g2_half8(r1, prefix & 7u) : g2_half8(r0, prefix & 7u);
                 uint32_t split = 0, bit = 0;
                 if (alive) bit = g2_bit(br, s_rcp, mw, split);
-                const uint32_t na = cnt_addr + ((uint32_t)max(idx - 1, 0) << 5) + ((prefix << 1) | bit);
-                const uint32_t mwn = (alive && idx > 0) ? model[na] : 0u;
-                G2_EMU_BARRIER();
+                const uint32_t p1 = (prefix << 1) | bit;
+                if (alive && idx == 5) r1 = *reinterpret_cast<const uint4*>(model + cnt_addr + (1u << 5) + (p1 << 3));
+                if (alive && idx == 4) r0 = *reinterpret_cast<const uint4*>(model + cnt_addr + (p1 << 3));
+                if (idx >= 4) G2_EMU_BARRIER();
                 if (alive) {
-                    model[a] = (uint16_t)g2_model_word(mw, bit);
+                    model[cnt_addr + ((uint32_t)idx << 5) + prefix] = (uint16_t)g2_model_word(mw, bit);
                     g2_update(br, split, bit);
-                    prefix = (prefix << 1) | bit;
+                    prefix = p1;
                 }
-                a = na; mw = mwn;
             }
             nz = (int)prefix;
             if (alive) nd += 6;
@@ -371,8 +396,6 @@ lep_decode_g2_kernel(const ImageDesc* __restrict__ images, SegDesc* __restrict__
                 const uint32_t eb = s_eb[ci][left_nz];
                 addr = eb + eoff[0];
                 a1 = addr + 1; a0 = eb + eoff[1];          // after the first exponent bit of position 0
-#pragma unroll
-                for (int k = 1; k <= G2_PF_DIST; ++k) g2_prefetch(model + eb + eoff[k]);        // positions 0..5 always exist
             }
             uint32_t mw = busy ? model[addr] : 0u;
             while (__any_sync(FULL, busy)) {
@@ -401,17 +424,6 @@ lep_decode_g2_kernel(const ImageDesc* __restrict__ images, SegDesc* __restrict__
                     const int nval = isS ? (1 << ((len - 1) & 31)) : (isR ? (val | ((int)bit << (ri & 31))) : val);
                     const bool nneg = isS ? !bit : neg;
                     if (evN && sub == 0) rcur[s_a2r[zz]] = (int16_t)(nneg ? -nval : nval);
-#if LEPB200_G2_PREFETCH
-                    if (isE & (int)bit & (int)(len == 0)) {       // non-zero: residual bits may follow, and the positions after it see one coefficient less
-                        g2_prefetch(model + m_resn(ci, s_a2r[zz], s_nzbin[left_nz]));
-                        const uint32_t eb1 = s_eb[ci][left_nz - 1];
-                        if (eb1 != s_eb[ci][left_nz] && left_nz > 1) {
-#pragma unroll
-                            for (int k = 1; k <= G2_PF_DIST; ++k) if (zz + k < 49) g2_prefetch(model + eb1 + eoff[zz + k]);
-                        }
-                    }
-                    if (ev && zz + 1 + G2_PF_DIST < 49) g2_prefetch(model + s_eb[ci][left_nz - evN] + eoff[zz + 1 + G2_PF_DIST]);
-#endif
                     left_nz -= evN; zz += ev;
                     st = toS ? G2_SIGN : toR ? G2_RES : ev ? G2_EXP : st;
                     len = ev ? 0 : len1;
@@ -459,9 +471,10 @@ lep_decode_g2_kernel(const ImageDesc* __restrict__ images, SegDesc* __restrict__
             eobx = colmask ? 31 - __clz(colmask) : 0;
             eoby = rowmask ? 31 - __clz(rowmask) : 0;
         }
+        G2EdgeTree eth = {}, etv = {};
         if (alive) {
-            g2_prefetch(model + m_nze(0, ci, eobx, (nz + 3) / 7, 0, 0));
-            g2_prefetch(model + m_nze(1, ci, eoby, (nz + 3) / 7, 0, 0));
+            eth = g2_edge_tree(model + m_nze(0, ci, eobx, (nz + 3) / 7, 0, 0));
+            etv = g2_edge_tree(model + m_nze(1, ci, eoby, (nz + 3) / 7, 0, 0));
             for (int k = sub; k < 14; k += G) {
                 int p = 0, coord;
                 if (k < 7) { coord = k + 1; if (has_above) p = lak_pred(rcur, rabove, icx + (k + 1) * 8, k + 1, 8); }
@@ -476,23 +489,20 @@ lep_decode_g2_kernel(const ImageDesc* __restrict__ images, SegDesc* __restrict__
         for (int vert = 0; vert < 2; ++vert) {
             int ne = 0;
             {
+                // the whole tree was read in (3): level idx is the row base + idx * 4, indexed by the bits above it
                 const uint32_t base = m_nze(vert, ci, vert ? eoby : eobx, (nz + 3) / 7, 0, 0);
-                uint32_t prefix = 0, a = base + (2u << 2);
-                uint32_t mw = alive ? model[a] : 0u;
-                G2_EMU_BARRIER();
-#pragma unroll 1
+                const G2EdgeTree t = vert ? etv : eth;
+                uint32_t prefix = 0;
+#pragma unroll
                 for (int idx = 2; idx >= 0; --idx) {
+                    const uint32_t mw = idx == 2 ? t.r2 : idx == 1 ? (t.r1 >> (prefix << 4)) & 0xffffu : g2_half4(t.r0, prefix);
                     uint32_t split = 0, bit = 0;
-                    if (alive) bit = g2_bit(br, s_rcp, mw, split);
-                    const uint32_t na = base + ((uint32_t)max(idx - 1, 0) << 2) + ((prefix << 1) | bit);
-                    const uint32_t mwn = (alive && idx > 0) ? model[na] : 0u;
-                    G2_EMU_BARRIER();
                     if (alive) {
-                        model[a] = (uint16_t)g2_model_word(mw, bit);
+                        bit = g2_bit(br, s_rcp, mw, split);
+                        model[base + ((uint32_t)idx << 2) + prefix] = (uint16_t)g2_model_word(mw, bit);
                         g2_update(br, split, bit);
                         prefix = (prefix << 1) | bit;
                     }
-                    a = na; mw = mwn;
                 }
                 ne = (int)prefix;
                 if (alive) nd += 3;
@@ -510,8 +520,6 @@ lep_decode_g2_kernel(const ImageDesc* __restrict__ images, SegDesc* __restrict__
                 addr = expx_base + (uint32_t)ne * NE_STRIDE + ((e & 15u) << 4);
                 a1 = addr + 1;
                 a0 = expx_base + (uint32_t)ne * NE_STRIDE + (uint32_t)(12 * 16) + ((einfo[vert * 7 + 1] & 15u) << 4);
-                g2_prefetch(model + a0);
-                g2_prefetch(model + expx_base + (uint32_t)ne * NE_STRIDE + (uint32_t)(2 * 12 * 16) + ((einfo[vert * 7 + 2] & 15u) << 4));
             }
             uint32_t mw = busy ? model[addr] : 0u;
             while (__any_sync(FULL, busy)) {
@@ -544,14 +552,6 @@ lep_decode_g2_kernel(const ImageDesc* __restrict__ images, SegDesc* __restrict__
                     const int nval = isS ? (1 << ((len - 1) & 31)) : ((isT | isR) ? (val | ((int)bit << (ri & 31))) : val);
                     const bool nneg = isS ? !bit : neg;
                     if (evN && sub == 0) rcur[(ln + 1) * cstep] = (int16_t)(nneg ? -nval : nval);
-#if LEPB200_G2_PREFETCH
-                    if (isE & (int)bit & (int)(len == 0) & (int)(ne > 1)) {      // non-zero: the next positions see one coefficient less
-                        if (ln < 6) g2_prefetch(model + expx_base + (uint32_t)(ne - 1) * NE_STRIDE + (uint32_t)((ln + 1) * (12 * 16)) + ((einfo[vert * 7 + ln + 1] & 15u) << 4));
-                        if (ln < 5) g2_prefetch(model + expx_base + (uint32_t)(ne - 1) * NE_STRIDE + (uint32_t)((ln + 2) * (12 * 16)) + ((einfo[vert * 7 + ln + 2] & 15u) << 4));
-                    }
-                    if (toS && len1 >= 2) g2_prefetch(model + (len1 - 2 >= mt ? m_thr(ci, (int)((e >> 9) & 255u), min(len1 - mt, 7)) : m_resn(ci, (ln + 1) * cstep, ne)));
-                    if (ev && ln + 3 < 7 && ne - evN > 0) g2_prefetch(model + expx_base + (uint32_t)(ne - evN) * NE_STRIDE + (uint32_t)((ln + 3) * (12 * 16)) + ((einfo[vert * 7 + ln + 3] & 15u) << 4));
-#endif
                     so = isT ? min((so << 1) | bit, 127u) : 1u;
                     thr_base = isS ? m_thr(ci, (int)((e >> 9) & 255u), min(len - mt, 7)) : thr_base;
                     ne -= evN; ln += ev;
@@ -658,7 +658,6 @@ lep_decode_g2_kernel(const ImageDesc* __restrict__ images, SegDesc* __restrict__
                 const int lm = min(bitlen((uint32_t)iabs(unc) & 0xffff), 11), lo16 = min(bitlen((uint32_t)iabs(unc2) & 0xffff), 16);
                 const int sctx = unc2 >= 0 ? (unc2 == 0 ? 3 : 2) : 1;
                 dc_exp = m_expdc(lm, lo16); dc_sign = m_sign(ci, 0, sctx); dc_res = m_resdc(lm);
-                g2_prefetch(model + dc_exp); g2_prefetch(model + dc_res);
             }
         }
 
@@ -728,11 +727,6 @@ lep_decode_g2_kernel(const ImageDesc* __restrict__ images, SegDesc* __restrict__
             }
             if (sub == 0) rnz[x] = (uint8_t)nz;
             nz_left = nz;
-            if (x + 1 < w) {              // the count of the next block of this row: its three model lines are known now
-                const int nza = has_above ? (int)rnz[x + 1] : 0;
-                const uint32_t a = m_nz7(ci, s_nzbin[has_above ? (nza + nz + 2) / 4 : (nz + 1) / 2], 0, 0);
-                g2_prefetch(model + a); g2_prefetch(model + a + 64); g2_prefetch(model + a + 128);
-            }
         }
         ndec += nd;
         if (bad) {                        // report the inconsistent stream; the group takes the next segment at the top
@@ -754,8 +748,15 @@ lep_decode_g2_kernel(const ImageDesc* __restrict__ images, SegDesc* __restrict__
                 dst[k] = lo | (hi << 16);
             }
             // a truncated image ends inside a row (component_size_in_blocks)
-            if (x + 1 >= w || (uint32_t)((size_t)y * w + x + 1) >= (uint32_t)gp->trunc_bc[c]) need_row = true;
-            else { ++x; pc ^= 1; pa ^= 1; }
+            if (x + 1 >= w || (uint32_t)((size_t)y * w + x + 1) >= (uint32_t)gp->trunc_bc[c]) {
+                need_row = true;
+            } else {                      // the 7x7 count tree of the next block is known now (phase (1b) with a left neighbour)
+                const int nza = has_above ? (int)rnz[x + 1] : 0;
+                cnt_addr = m_nz7(ci, s_nzbin[has_above ? (nza + nz + 2) / 4 : (nz + 1) / 2], 0, 0);
+                nzt = g2_nz_top(model + cnt_addr);
+                cnt_ready = true;
+                ++x; pc ^= 1; pa ^= 1;
+            }
         }
         __syncwarp();
     }
