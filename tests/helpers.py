@@ -108,6 +108,27 @@ def truncated_cut_of(lep_name):
     return truncated_source(e["source"])[:e["cut"]]
 
 
+# baseline JPEGs with every sampling geometry the reference accepts and what the reference CLI made of them
+# (tests/golden/make_geometry.py)
+GEOMETRY = json.load(open(os.path.join(GOLDEN, "geometry.json")))
+
+
+def geometry_jpegs():
+    return sorted(n for n in GEOMETRY if n.endswith(".jpg"))
+
+
+def geometry_leps():
+    """(name of the .lep, name of its source JPEG) for every reference-written .lep of the geometry corpus: one per
+    accepted JPEG plus the multi-segment records."""
+    out = [(n[:-4] + ".lep", n) for n in geometry_jpegs() if GEOMETRY[n]["status_want"] == 0]
+    out += [(n, e["source"]) for n, e in GEOMETRY.items() if n.endswith(".lep")]
+    return sorted(out)
+
+
+def load_geometry_lep(name):
+    return lepfmt.parse_container(read_golden("geometry/" + name))
+
+
 def geometry_of(lf):
     f = lf.frame
     tbcv, tbc = lepfmt.truncation(lf)
