@@ -185,6 +185,11 @@ int lepb200_huffman_encode_fetch(lepb200_ctx* ctx, lepb200_henc_image* images, i
 int lepb200_huffman_encode_resident_parts(lepb200_ctx* ctx, lepb200_henc_image* images, int nimages, int nparts);
 int lepb200_huffman_encode_parts(const lepb200_ctx* ctx);
 int lepb200_huffman_encode_wait_part(lepb200_ctx* ctx, lepb200_henc_image* images, int nimages, int part, int* first, int* last);
+/* Adler-32 (RFC 1950) of the scan bytes of images [first, last) of the batch, taken by the encode kernel while it wrote them
+ * (each warp over its thread-segment; the segments are combined here in order): adler[i] for i in [first, last).  Valid for
+ * images whose part lepb200_huffman_encode_wait_part returned, or after lepb200_huffman_encode_fetch; meaningful where the
+ * image's status is 0.  A skipped image (scan_bytes == 0) gets 1, the Adler-32 of no bytes. */
+int lepb200_huffman_encode_adler32(lepb200_ctx* ctx, int first, int last, uint32_t* adler);
 /* Per-segment status of the decode batch as soon as the decode kernel has finished (a second stream: work queued behind
  * the kernel -- the Huffman encode above -- is not waited for).  lepb200_decode_fetch reports the same later. */
 int lepb200_decode_fetch_status(lepb200_ctx* ctx, int32_t* status_out);
@@ -265,6 +270,13 @@ void lepb200_codec_set_encode_threads(lepb200_codec* codec, int min_threads, int
 void lepb200_codec_set_verify(lepb200_codec* codec, int on);
 /* -evensplit (jpgcoder.cc:1063-1064, :3898-3900): thread-segments cover equal numbers of MCU rows instead of equal bytes */
 void lepb200_codec_set_even_split(lepb200_codec* codec, int on);
+/* -zlib0 (jpgcoder.cc:2089, check_file :2200-2220, src/io/Zlib0.cc): 1 = lepb200_decompress_leps hands every restored JPEG out
+ * as a zlib stream: 78 01, stored deflate blocks of 65535 bytes (the last one BFINAL and never empty), the big-endian Adler-32
+ * of the JPEG -- 2 + n + 5 ceil(n / 65535) + 4 bytes for an n-byte JPEG.  Files whose magic is CE B6 (zeta) instead of CF 84
+ * are always handed out so, whatever this setting.  The Adler-32 of a scan the device re-encodes is taken by the encode kernel
+ * (environment LEPB200_ZLIB0_HOST_ADLER=1: by the host, over every byte).  Statuses do not change; lepb200_compress_jpegs
+ * ignores the setting, as the reference does.  0 (default): plain JPEG bytes. */
+void lepb200_codec_set_zlib0(lepb200_codec* codec, int on);
 /* device milliseconds of the last chunk's GPU Huffman-decode kernel (diagnostic) */
 double lepb200_codec_last_huffman_ms(const lepb200_codec* codec);
 /* files of the last lepb200_decompress_leps call whose scan was Huffman-encoded on the device (the rest went through the host re-encoder) */
@@ -326,6 +338,11 @@ int lepb200_host_lep_lazy_equal(const uint8_t* data, size_t len);
 int lepb200_host_lep_henc_image(lepb200_lep* h, lepb200_henc_image* out);
 int lepb200_host_lep_assemble(lepb200_lep* h, const uint8_t* scan, size_t scan_len, const uint8_t** data, size_t* len);
 void lepb200_host_lep_close(lepb200_lep* h);
+/* 1 when the container opened with lepb200_host_lep_open carries the zeta magic CE B6 (its JPEG is restored as a zlib stream) */
+int lepb200_host_lep_zlib0(const lepb200_lep* h);
+/* test hook: the zlib stream lepb200_codec_set_zlib0 hands out for the `len` bytes at `data`.  Returns its length; writes it
+ * to `out` only when cap is at least that length. */
+size_t lepb200_host_zlib0_frame(const uint8_t* data, size_t len, uint8_t* out, size_t cap);
 /* diagnostic: wall-clock seconds of the host front end alone over a batch with `threads` workers */
 double lepb200_host_frontend_seconds(const lepb200_buffer* jpegs, int n, int threads, int32_t* first_error);
 

@@ -63,6 +63,7 @@ _EXPORTS = [
     "lepb200_host_jpeg_error", "lepb200_host_jpeg_image", "lepb200_host_jpeg_scan", "lepb200_last_huffman_iterations", "lepb200_huffman_encode_resident_parts", "lepb200_huffman_encode_parts", "lepb200_huffman_encode_wait_part", "lepb200_decode_fetch_status", "lepb200_decode_upload_gather", "lepb200_encode_fetch_files", "lepb200_host_jpeg_write_lep", "lepb200_host_jpeg_header", "lepb200_host_mux_plan", "lepb200_host_lep_henc_image", "lepb200_host_brotli_available", "lepb200_host_lep_lazy_equal", "lepb200_host_jpeg_close",
     "lepb200_decompress_leps", "lepb200_host_lep_open", "lepb200_host_lep_error", "lepb200_host_lep_image",
     "lepb200_host_lep_stream", "lepb200_host_lep_recode", "lepb200_host_lep_close", "lepb200_host_frontend_seconds",
+    "lepb200_codec_set_zlib0", "lepb200_huffman_encode_adler32", "lepb200_host_lep_zlib0", "lepb200_host_zlib0_frame",
 ]
 
 
@@ -353,6 +354,12 @@ def _bind_file_api(L):
     L.lepb200_codec_set_even_split.restype = None
     L.lepb200_codec_set_verify.argtypes = [vp, ctypes.c_int]
     L.lepb200_codec_set_verify.restype = None
+    L.lepb200_codec_set_zlib0.argtypes = [vp, ctypes.c_int]
+    L.lepb200_codec_set_zlib0.restype = None
+    L.lepb200_host_lep_zlib0.argtypes = [vp]
+    L.lepb200_host_lep_zlib0.restype = ctypes.c_int
+    L.lepb200_host_zlib0_frame.argtypes = [ctypes.c_char_p, ctypes.c_size_t, ctypes.c_void_p, ctypes.c_size_t]
+    L.lepb200_host_zlib0_frame.restype = ctypes.c_size_t
     L.lepb200_host_jpeg_error.argtypes = [vp]
     L.lepb200_host_jpeg_error.restype = ctypes.c_char_p
     L.lepb200_host_jpeg_image.argtypes = [vp, ctypes.POINTER(_Image)]
@@ -475,6 +482,11 @@ class HostLep:
                          trunc_bcv=[im.trunc_bcv[c] for c in range(im.ncmp)],
                          trunc_bc=[im.trunc_bc[c] for c in range(im.ncmp)])
 
+    @property
+    def zlib0(self) -> bool:
+        """True for a container with the zeta magic (CE B6): its JPEG is restored as a zlib stream."""
+        return bool(self._L.lepb200_host_lep_zlib0(self._h))
+
     def scan_layout(self):
         """(offset, length) of the entropy-coded scan in the original JPEG, (0, 0) if the host has to re-encode it."""
         off, n = ctypes.c_uint32(), ctypes.c_uint32()
@@ -511,12 +523,23 @@ class HostLep:
         return ctypes.string_at(d, n.value)
 
 
+def zlib0_frame(data: bytes) -> bytes:
+    """The zlib stream of stored blocks that decompress(..) hands out for these bytes with zlib0=True (host code, no GPU)."""
+    L = lib()
+    _bind_file_api(L)
+    n = L.lepb200_host_zlib0_frame(data, len(data), None, 0)
+    out = ctypes.create_string_buffer(n)
+    assert L.lepb200_host_zlib0_frame(data, len(data), out, n) == n
+    return out.raw
+
+
 class LeptonB200FileCodec:
-    """JPEG bytes -> .lep bytes for a batch of files; host threads + one GPU."""
+    """JPEG bytes -> .lep bytes for a batch of files; host threads + one GPU.  zlib0=True (-zlib0): decompress hands every
+    JPEG out as a zlib stream of stored blocks, as containers with the zeta magic (CE B6) always are."""
 
     def __init__(self, device: int = 0, host_threads: int = 0, chunk_images: int = 0, gpu_huffman: bool = True,
                  allow_progressive: bool = True, min_encode_threads: int = 1, max_encode_threads: int = 8,
-                 even_split: bool = False, verify: bool = False):
+                 even_split: bool = False, verify: bool = False, zlib0: bool = False):
         self._L = lib()
         _bind_file_api(self._L)
         self._c = ctypes.c_void_p()
@@ -530,6 +553,7 @@ class LeptonB200FileCodec:
         self._L.lepb200_codec_set_encode_threads(self._c, min_encode_threads, max_encode_threads)   # -minencodethreads= / -maxencodethreads=
         self._L.lepb200_codec_set_even_split(self._c, 1 if even_split else 0)                      # -evensplit
         self._L.lepb200_codec_set_verify(self._c, 1 if verify else 0)                              # -verify (reference default) / -skipverify
+        self._L.lepb200_codec_set_zlib0(self._c, 1 if zlib0 else 0)                                # -zlib0
 
     def close(self):
         if self._c:

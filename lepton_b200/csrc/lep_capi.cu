@@ -9,6 +9,8 @@
 #include <tuple>
 #include <vector>
 
+#include <zlib.h>
+
 #include "../../include/lepton_b200.h"
 #include "lep_common.cuh"
 #include "lep_predict.cuh"
@@ -87,6 +89,7 @@ struct lepb200_ctx {
     bool status_queued = false;
     std::vector<size_t> henc_off;         // per image: offset of its scan bytes in the output buffers (SIZE_MAX = skipped)
     std::vector<int> henc_seg_first;      // per image: index of its first segment record
+    std::vector<int> henc_seg_count;      // per image: its number of segment records
     int henc_nseg = 0;
     // parts of the last lepb200_huffman_encode_resident_parts call: image range, segment range, byte range of the output,
     // the event behind the part's D2H copies on copy_stream
@@ -1014,6 +1017,7 @@ static int henc_launch(lepb200_ctx* ctx, lepb200_henc_image* imgs, int n, int np
     };
     ctx->henc_off.assign(n, SIZE_MAX);
     ctx->henc_seg_first.assign(n, -1);
+    ctx->henc_seg_count.assign(n, 0);
     size_t total = 0;
     for (int i = 0; i < n; ++i) {
         lepb200_henc_image& im = imgs[i];
@@ -1036,6 +1040,7 @@ static int henc_launch(lepb200_ctx* ctx, lepb200_henc_image* imgs, int n, int np
         if (!ok) { im.status = LEPB200_ST_NOT_HANDLED; im.scan_bytes = 0; continue; }
         ctx->henc_off[i] = total;
         ctx->henc_seg_first[i] = (int)hs.size();
+        ctx->henc_seg_count[i] = im.nseg;
         uint32_t off = 0;
         for (int k = 0; k < im.nseg; ++k) {
             HEncSeg sg;
@@ -1174,6 +1179,20 @@ int lepb200_huffman_encode_fetch(lepb200_ctx* ctx, lepb200_henc_image* imgs, int
         int st = 0;
         for (int k = 0; k < imgs[i].nseg; ++k) if (hs[ctx->henc_seg_first[i] + k].status) st = 1;
         imgs[i].status = st;
+    }
+    return LEPB200_OK;
+}
+
+int lepb200_huffman_encode_adler32(lepb200_ctx* ctx, int first, int last, uint32_t* adler) {
+    if (!ctx || !adler || first < 0 || first > last || last > (int)ctx->henc_off.size()) return LEPB200_ERR_INVALID;
+    const HEncSeg* hs = static_cast<const HEncSeg*>(ctx->h_henc_segs.p);
+    for (int i = first; i < last; ++i) {
+        uLong a = adler32(0L, Z_NULL, 0);
+        for (int k = 0; ctx->henc_off[i] != SIZE_MAX && k < ctx->henc_seg_count[i]; ++k) {     // segments lie back to back, in order
+            const HEncSeg& sg = hs[ctx->henc_seg_first[i] + k];
+            a = adler32_combine(a, sg.adler, (z_off_t)sg.produced);
+        }
+        adler[i] = (uint32_t)a;
     }
     return LEPB200_OK;
 }

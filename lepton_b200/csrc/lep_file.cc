@@ -41,6 +41,7 @@ struct lepb200_codec {
     unsigned max_encode_threads = 8, min_encode_threads = 1;   // -maxencodethreads= / -minencodethreads= (jpgcoder.cc:1080-1089)
     bool verify = false;           // -verify: decode every .lep again and compare with the input before handing it out
     bool allow_progressive = true; // false: -rejectprogressive (files that are not single-scan-interleaved baseline exit with code 8)
+    bool zlib0 = false;            // -zlib0: restored JPEGs are handed out as zlib streams of stored blocks
     void* arena[4] = {nullptr, nullptr, nullptr, nullptr};  // pinned host memory for coefficient planes, one per in-flight chunk
     size_t arena_cap[4] = {0, 0, 0, 0};
     std::vector<std::vector<uint8_t>> outputs;
@@ -154,6 +155,7 @@ void lepb200_codec_set_gpu_huffman(lepb200_codec* c, int on) { if (c) c->gpu_huf
 void lepb200_codec_set_allow_progressive(lepb200_codec* c, int on) { if (c) c->allow_progressive = on != 0; }
 void lepb200_codec_set_even_split(lepb200_codec* c, int on) { if (c) c->even_split = on != 0; }
 void lepb200_codec_set_verify(lepb200_codec* c, int on) { if (c) c->verify = on != 0; }
+void lepb200_codec_set_zlib0(lepb200_codec* c, int on) { if (c) c->zlib0 = on != 0; }
 void lepb200_codec_set_encode_threads(lepb200_codec* c, int min_threads, int max_threads) {
     if (!c) return;
     c->min_encode_threads = (unsigned)std::min(std::max(min_threads, 1), 8);
@@ -525,7 +527,10 @@ int lepb200_compress_jpegs(lepb200_codec* c, const lepb200_buffer* jpegs, int n,
         if (!idx.empty()) {
             const double tf = c->t_front, tg = c->t_gpu, tb = c->t_back;
             std::vector<lepb200_result> back(idx.size(), lepb200_result{nullptr, 0, 0});
+            const bool zlib0 = c->zlib0;                                         // the check compares plain JPEG bytes
+            c->zlib0 = false;
             const int vrc = lepb200_decompress_leps(c, vin.data(), (int)vin.size(), back.data());
+            c->zlib0 = zlib0;
             for (size_t q = 0; q < idx.size(); ++q) {
                 const lepb200_buffer& src = jpegs[idx[q]];
                 const bool same = vrc == LEPB200_OK && back[q].status == 0 && back[q].len == src.len && !memcmp(back[q].data, src.data, src.len);
@@ -717,6 +722,13 @@ int lepb200_decompress_leps(lepb200_codec* c, const lepb200_buffer* leps, int n,
     // parts of the device Huffman encode whose D2H and JPEG assembly run under the encode of the next part
     // (LEPB200_HENC_PARTS, 1 = one launch, everything after it as before round 2's last change)
     const int henc_parts_want = getenv("LEPB200_HENC_PARTS") ? std::max(1, std::min(16, atoi(getenv("LEPB200_HENC_PARTS")))) : 4;
+    // zlib0 output (codec setting, or a zeta-headed file): the Adler-32 of a device-encoded scan comes from the encode kernel
+    // unless LEPB200_ZLIB0_HOST_ADLER=1, which has the host sum every byte (the route of host-encoded files) for comparison
+    const bool zlib0_host_adler = getenv("LEPB200_ZLIB0_HOST_ADLER") && atoi(getenv("LEPB200_ZLIB0_HOST_ADLER")) != 0;
+    auto out_mode = [&](const LepFile& lf, bool device_scan) {
+        if (!c->zlib0 && !lf.zlib0) return JpegOut::plain;
+        return device_scan && !zlib0_host_adler ? JpegOut::zlib0_scan_adler : JpegOut::zlib0_host_adler;
+    };
     auto gpu = [&](int k) {               // H2D of the streams + decode kernel + Huffman encode of the resident planes, all queued
         double t0 = now_s();
         DChunk& s = cs[k];
@@ -732,19 +744,23 @@ int lepb200_decompress_leps(lepb200_codec* c, const lepb200_buffer* leps, int n,
         c->t_gpu += now_s() - t0;
     };
     // JPEG of one batch image from the scan the device produced
-    auto assemble = [&](DChunk& s, int q) {
+    auto assemble = [&](DChunk& s, int q, uint32_t scan_adler) {
         const int li = s.idx[q], i = s.begin + li;
         for (int t = s.seg_base[q]; t < s.seg_base[q + 1]; ++t)
             if (s.seg_status[t]) { status[i] = s.seg_status[t]; return; }
         std::string err;
         c->n_gpu_recoded++;
-        if (!assemble_baseline(*s.lf[li], s.gsetup[q], s.henc[q].data, c->outputs[i], err)) { status[i] = NOT_HANDLED; c->outputs[i].clear(); }
+        const LepFile& lf = *s.lf[li];
+        if (!assemble_baseline(lf, s.gsetup[q], s.henc[q].data, c->outputs[i], err, out_mode(lf, true), scan_adler)) { status[i] = NOT_HANDLED; c->outputs[i].clear(); }
     };
     auto fetch_back = [&](int k) {
         double t0 = now_s();
         DChunk& s = cs[k];
         const int nb = (int)s.imgs.size();
         std::vector<uint8_t> done(nb, 0);
+        std::vector<uint32_t> scan_adler(nb, 1);
+        bool kernel_adler = false;                      // some file of the chunk takes its scan's Adler-32 from the encode kernel
+        for (int q = 0; q < nb; ++q) kernel_adler |= out_mode(*s.lf[s.idx[q]], true) == JpegOut::zlib0_scan_adler;
         lepb200_ctx* ctx = nb ? c->ctx2[k % W] : nullptr;
         if (s.gpu_rc == 0 && nb) {
             // decode status as soon as the decode kernel is through, then the parts of the device re-encode as they arrive
@@ -755,6 +771,7 @@ int lepb200_decompress_leps(lepb200_codec* c, const lepb200_buffer* leps, int n,
                 double tp = now_s();
                 int q0 = 0, q1 = 0;
                 s.gpu_rc = lepb200_huffman_encode_wait_part(ctx, s.henc.data(), nb, p, &q0, &q1);
+                if (s.gpu_rc == 0 && kernel_adler) s.gpu_rc = lepb200_huffman_encode_adler32(ctx, q0, q1, scan_adler.data());
                 if (s.gpu_rc) break;
                 mark("huffenc part", k, tp);
                 tp = now_s();
@@ -762,7 +779,7 @@ int lepb200_decompress_leps(lepb200_codec* c, const lepb200_buffer* leps, int n,
                     const int q = q0 + d;
                     const lepb200_henc_image& he = s.henc[q];
                     if (!(he.scan_bytes && he.status == 0 && he.data)) return;
-                    assemble(s, q);
+                    assemble(s, q, scan_adler[q]);
                     done[q] = 1;
                 });
                 mark("assemble part", k, tp);
@@ -797,7 +814,8 @@ int lepb200_decompress_leps(lepb200_codec* c, const lepb200_buffer* leps, int n,
                 for (int t = s.seg_base[q]; t < s.seg_base[q + 1]; ++t)
                     if (s.seg_status[t]) { status[i] = s.seg_status[t]; return; }
                 std::string err;
-                if (!recode_baseline(*s.lf[li], s.planes[li].data(), c->outputs[i], err)) { status[i] = NOT_HANDLED; c->outputs[i].clear(); }
+                const LepFile& lf = *s.lf[li];
+                if (!recode_baseline(lf, s.planes[li].data(), c->outputs[i], err, out_mode(lf, false))) { status[i] = NOT_HANDLED; c->outputs[i].clear(); }
             });
         }
         s.lf.clear();
@@ -913,6 +931,17 @@ int lepb200_host_lep_assemble(lepb200_lep* h, const uint8_t* scan, size_t scan_l
     return LEPB200_OK;
 }
 void lepb200_host_lep_close(lepb200_lep* h) { delete h; }
+int lepb200_host_lep_zlib0(const lepb200_lep* h) { return h && h->lf.zlib0 ? 1 : 0; }
+size_t lepb200_host_zlib0_frame(const uint8_t* data, size_t len, uint8_t* out, size_t cap) {
+    if (!data && len) return 0;
+    const size_t need = zlib0_size(len);
+    if (out && cap >= need) {
+        std::vector<uint8_t> framed;
+        zlib0_frame(data, len, framed);
+        memcpy(out, framed.data(), need);
+    }
+    return need;
+}
 
 // Host front end only (parse + Huffman decode + split selection) over a batch with `threads` workers; returns the
 // wall-clock seconds.  Diagnostic: lets the host stage be profiled without a GPU.

@@ -34,11 +34,13 @@ struct HEncSeg {
     int32_t is_last;
     int32_t status;                  // out: 0 ok, 1 length mismatch
     uint32_t produced;               // out
+    uint32_t adler;                  // out: Adler-32 (RFC 1950) of the bytes written, [out_off, out_off + produced)
 };
 
 constexpr int HENC_WARPS = 4;
 constexpr int HENC_WORDS = 160;      // bit buffer per warp: flushed once it holds HENC_FLUSH_BITS; a block adds at most ~1800 bits
 constexpr uint32_t HENC_FLUSH_BITS = 2560;
+constexpr uint32_t ADLER_MOD = 65521;
 
 static __constant__ uint8_t c_zz2al[64] = {
     49, 50, 57, 58, 0, 51, 52, 1, 2, 59, 60, 3, 4, 5, 53, 54, 6, 7, 8, 9, 61, 62, 10, 11,
@@ -91,6 +93,10 @@ lep_huffencode_kernel(const HEncImage* __restrict__ images, HEncSeg* __restrict_
     int rstw = 0, cpos = 0;
     if (rsti > 0) { const int m0 = sg.my0 * mcuh; rstw = rsti - (m0 % rsti); cpos = m0 / rsti; }
     const int mcu_end = im.mcuv * mcuh;
+    // Adler-32 of the written bytes, taken while they are in registers: each lane sums the bytes it writes (a) and each byte
+    // times its position relative to out_off (p); stuffed zeros add nothing.  p is reduced once per flush (a lane adds at most
+    // about 20 terms below 2^40 between reductions), a at the end (below 2^40 for any 32-bit segment length).
+    unsigned long long ad_a = 0, ad_p = 0;
 
     // writes the complete bytes of the buffer (with 0xFF stuffing) and keeps the remaining bits
     auto flush = [&]() {
@@ -102,11 +108,12 @@ lep_huffencode_kernel(const HEncImage* __restrict__ images, HEncSeg* __restrict_
             const uint32_t ffm = __ballot_sync(FULL, act && b == 0xffu);
             const uint32_t dst = opos + (i - base) + __popc(ffm & ((1u << lane) - 1));
             if (act) {
-                if (dst < limit) out[dst] = (uint8_t)b;
+                if (dst < limit) { out[dst] = (uint8_t)b; ad_a += b; ad_p += (unsigned long long)(dst - sg.out_off) * b; }
                 if (b == 0xffu && dst + 1 < limit) out[dst + 1] = 0;
             }
             opos += min(32u, nbytes - base) + __popc(ffm);
         }
+        ad_p %= ADLER_MOD;
         __syncwarp();
         // move the leftover bits to the front, clear the rest
         const uint32_t rem = nbit & 7;
@@ -204,8 +211,9 @@ lep_huffencode_kernel(const HEncImage* __restrict__ images, HEncSeg* __restrict_
                 }
                 flush();                                                  // every pending byte goes out before the marker
                 if (lane == 0) {
-                    if (opos < limit) out[opos] = 0xFF;
-                    if (opos + 1 < limit) out[opos + 1] = (uint8_t)(0xD0 + (cpos & 7));
+                    const uint32_t mk = 0xD0u + (cpos & 7), rel = opos - sg.out_off;
+                    if (opos < limit) { out[opos] = 0xFF; ad_a += 0xFFu; ad_p += (unsigned long long)rel * 0xFFu; }
+                    if (opos + 1 < limit) { out[opos + 1] = (uint8_t)mk; ad_a += mk; ad_p += (unsigned long long)(rel + 1) * mk; }
                 }
                 opos += 2;
                 ++cpos;
@@ -223,9 +231,16 @@ lep_huffencode_kernel(const HEncImage* __restrict__ images, HEncSeg* __restrict_
         __syncwarp();
     }
     flush();                                                              // complete bytes; a non-last segment drops its last bits (the next one starts with them)
+    ad_a = __reduce_add_sync(FULL, (unsigned)(ad_a % ADLER_MOD));           // 32 terms below 2^16 each
+    ad_p = __reduce_add_sync(FULL, (unsigned)ad_p);
     if (lane == 0) {
         const uint32_t produced = opos - sg.out_off;
         sg.produced = produced;
+        // bytes b_0 .. b_{n-1}: A = 1 + sum b_i, B = n + sum (n - i) b_i = n + n (A - 1) - sum i b_i  (mod 65521)
+        const unsigned long long n = produced % ADLER_MOD, a = ad_a % ADLER_MOD, p = ad_p % ADLER_MOD;
+        const uint32_t A = (uint32_t)((1 + a) % ADLER_MOD);
+        const uint32_t B = (uint32_t)((n + n * a + ADLER_MOD - p) % ADLER_MOD);
+        sg.adler = (B << 16) | A;
         const uint32_t want = sg.is_last ? limit - sg.out_off : sg.expect;
         sg.status = produced == want ? 0 : 1;
     }

@@ -83,7 +83,11 @@ const uint8_t k_zigzag_to_aligned[64] = {
 bool brotli_available() { return brotli_api().ok; }
 
 bool read_lep(const uint8_t* d, size_t n, LepFile& lf, bool lazy) {
-    if (n < 28 + 3 + 4 || d[0] != 0xCF || d[1] != 0x84) return lfail(lf, VERSION_UNSUPPORTED, "not a .lep file");
+    // CF 84 (tau): the usual container; CE B6 (zeta, zlepton_header, jpgcoder.cc:552): the same container whose JPEG is handed
+    // out as a zlib stream (check_file, jpgcoder.cc:2200-2220)
+    const bool zeta = n >= 2 && d[0] == 0xCE && d[1] == 0xB6;
+    if (n < 28 + 3 + 4 || !((d[0] == 0xCF && d[1] == 0x84) || zeta)) return lfail(lf, VERSION_UNSUPPORTED, "not a .lep file");
+    lf.zlib0 = zeta;
     lf.version = d[2]; lf.flag = d[3]; lf.nseg = d[4];
     // version 1: zlib header blob; 2 and 4: brotli header blob (and an EOF marker behind the mux packets); 3: brotli header AND the
     // ANS coder instead of the bool coder (makeDecoder(..., ujgversion == 3), jpgcoder.cc:1727) -- another codec, refused
@@ -450,25 +454,99 @@ bool gpu_recode_setup(const LepFile& lf, GpuRecodeSetup& out) {
     return true;
 }
 
-bool assemble_baseline(const LepFile& lf, const GpuRecodeSetup& gs, const uint8_t* scan, std::vector<uint8_t>& out, std::string& err) {
+namespace {
+constexpr size_t ZLIB0_BLOCK = 65535;
+
+// Writes the zlib0 stream of a payload of known length `n` that arrives in pieces: block headers go in where the payload
+// crosses a block boundary, so every payload byte is copied exactly once.
+struct Zlib0Writer {
+    uint8_t* q = nullptr;
+    size_t n = 0, pos = 0;            // payload length, payload bytes written so far
+    bool sum = false;                 // take the Adler-32 of the pieces here
+    uLong adler = 1;
+    Zlib0Writer(std::vector<uint8_t>& out, size_t len, bool take_adler) : n(len), sum(take_adler) {
+        out.resize(zlib0_size(len));
+        q = out.data();
+        *q++ = 0x78; *q++ = 0x01;     // CMF: deflate, 32 K window; FLG: no dictionary, fastest (check bits: 0x7801 % 31 == 0)
+        if (n == 0) { *q++ = 1; *q++ = 0; *q++ = 0; *q++ = 0xFF; *q++ = 0xFF; }     // nothing to store: one empty final block
+    }
+    void put(const uint8_t* p, size_t len) {
+        if (sum) adler = adler32(adler, p, (uInt)len);
+        while (len) {
+            if (pos % ZLIB0_BLOCK == 0) {
+                const size_t b = std::min(ZLIB0_BLOCK, n - pos);
+                q[0] = pos + b == n ? 1 : 0;
+                q[1] = (uint8_t)b; q[2] = (uint8_t)(b >> 8); q[3] = (uint8_t)~b; q[4] = (uint8_t)(~b >> 8);
+                q += 5;
+            }
+            const size_t k = std::min(len, ZLIB0_BLOCK - pos % ZLIB0_BLOCK);
+            memcpy(q, p, k);
+            q += k; p += k; pos += k; len -= k;
+        }
+    }
+    void finish(uint32_t a) { q[0] = (uint8_t)(a >> 24); q[1] = (uint8_t)(a >> 16); q[2] = (uint8_t)(a >> 8); q[3] = (uint8_t)a; }
+};
+}  // namespace
+
+size_t zlib0_size(size_t n) { return 2 + n + 5 * std::max<size_t>(1, (n + ZLIB0_BLOCK - 1) / ZLIB0_BLOCK) + 4; }
+
+void zlib0_frame(const uint8_t* data, size_t n, std::vector<uint8_t>& out) {
+    Zlib0Writer w(out, n, true);
+    w.put(data, n);
+    w.finish((uint32_t)w.adler);
+}
+
+bool assemble_baseline(const LepFile& lf, const GpuRecodeSetup& gs, const uint8_t* scan, std::vector<uint8_t>& out, std::string& err,
+                       JpegOut mode, uint32_t scan_adler) {
     const Jpeg& j = lf.j;
     const std::vector<uint8_t>& h = j.hdr;
-    out.clear();
-    out.reserve((size_t)lf.jpeg_size + 16);
-    out.push_back(0xFF); out.push_back(0xD8);
-    out.insert(out.end(), h.begin(), h.begin() + gs.hpos);
-    out.insert(out.end(), scan, scan + gs.scan_bytes);
+    static const uint8_t soi[2] = {0xFF, 0xD8};
+    uint8_t rst[2 * 256];                                  // trailing restart markers (rst_err entries are bytes)
+    size_t nrst = 0;
     if (!j.rst_err.empty()) {
         const unsigned cum = gs.rsti ? (unsigned)(j.mcuh * j.mcuv - 1) / gs.rsti : 0;
-        for (unsigned i = 0; i < j.rst_err[0]; ++i) { out.push_back(0xFF); out.push_back((uint8_t)(0xD0 + ((cum + i) & 7))); }
+        for (unsigned i = 0; i < j.rst_err[0] && nrst + 2 <= sizeof(rst); ++i) { rst[nrst++] = 0xFF; rst[nrst++] = (uint8_t)(0xD0 + ((cum + i) & 7)); }
     }
-    out.insert(out.end(), h.begin() + gs.hpos, h.end());
-    out.insert(out.end(), j.grb.begin(), j.grb.end());
-    if (out.size() != lf.jpeg_size) { err = "re-created JPEG has the wrong size"; return false; }
+    // the JPEG in pieces: [0, 2) in front of the scan, [2] the scan, [3, 6) behind it
+    const std::pair<const uint8_t*, size_t> pieces[6] = {
+        {soi, 2}, {h.data(), gs.hpos}, {scan, gs.scan_bytes}, {rst, nrst}, {h.data() + gs.hpos, h.size() - gs.hpos}, {j.grb.data(), j.grb.size()}};
+    size_t total = 0;
+    for (const auto& pc : pieces) total += pc.second;
+    if (total != lf.jpeg_size) { err = "re-created JPEG has the wrong size"; out.clear(); return false; }
+    if (mode == JpegOut::plain) {
+        out.clear();
+        out.reserve((size_t)lf.jpeg_size + 16);
+        for (const auto& pc : pieces) out.insert(out.end(), pc.first, pc.first + pc.second);
+        return true;
+    }
+    const bool host_sum = mode == JpegOut::zlib0_host_adler;
+    Zlib0Writer w(out, total, host_sum);
+    if (host_sum) {
+        for (const auto& pc : pieces) w.put(pc.first, pc.second);
+        w.finish((uint32_t)w.adler);
+        return true;
+    }
+    // the device took the scan's sum; the host sums the few header and trailer bytes and combines the three
+    uLong head = 1, tail = 1;
+    size_t ntail = 0;
+    for (int k = 0; k < 6; ++k) {
+        w.put(pieces[k].first, pieces[k].second);
+        if (k < 2) head = adler32(head, pieces[k].first, (uInt)pieces[k].second);
+        if (k > 2) { tail = adler32(tail, pieces[k].first, (uInt)pieces[k].second); ntail += pieces[k].second; }
+    }
+    uLong a = adler32_combine(head, scan_adler, (z_off_t)gs.scan_bytes);
+    a = adler32_combine(a, tail, (z_off_t)ntail);
+    w.finish((uint32_t)a);
     return true;
 }
 
-bool recode_baseline(const LepFile& lf, const int16_t* const planes[4], std::vector<uint8_t>& out, std::string& err) {
+bool recode_baseline(const LepFile& lf, const int16_t* const planes[4], std::vector<uint8_t>& out, std::string& err, JpegOut mode) {
+    if (mode != JpegOut::plain) {
+        thread_local std::vector<uint8_t> jpeg;
+        if (!recode_baseline(lf, planes, jpeg, err, JpegOut::plain)) { out.clear(); return false; }
+        zlib0_frame(jpeg.data(), jpeg.size(), out);
+        return true;
+    }
     const Jpeg& j = lf.j;
     if (lf.flag != 'Z' || j.jpegtype != 1) return recode_scans(lf, planes, out, err);     // multi-scan / progressive files
     const std::vector<uint8_t>& h = j.hdr;

@@ -2,20 +2,23 @@
 //
 // Keeps the part of the reference CLI surface that selects what is computed (src/lepton/jpgcoder.cc
 // initialize_options :988-1219, process_file :1528): `lepton [flags] <in.jpg|in.lep> [out]`, direction chosen from
-// the first two bytes of the input (FF D8 -> compress, CF 84 -> decompress; check_file :2178), `-` for stdin/stdout,
+// the first two bytes of the input (FF D8 -> compress, CF 84 or CE B6 -> decompress; check_file :2178), `-` for stdin/stdout,
 // exit status = the reference's ExitCode (src/vp8/util/memory.hh:13-39).  Flags that only configure the reference's
 // CPU runtime (-singlethread, -unjailed, -preload, -memory=, -threadmemory=, -timebound=) are accepted and ignored.
 // Like the reference, the CLI verifies every .lep it writes by decoding it again (exit code 41, ROUNDTRIP_FAILURE, and no
 // output when the input does not come back byte for byte) unless -skipverify is given.  Service modes (-socket, -listen, -fork,
-// -benchmark, -lepcat) and output variants this build does not write (-brotliheader, -ans, -zlib0, -ujg, -startbyte /
-// -trunc slices, -embedding) are refused, never silently ignored.  Flags that change the bytes are honoured:
-// -minencodethreads= / -maxencodethreads= / -evensplit (thread-segment selection), -rejectprogressive / -allowprogressive.
+// -benchmark, -lepcat) and output variants this build does not write (-brotliheader, -ans, -ujg, -startbyte / -trunc slices,
+// -embedding) are refused, never silently ignored.  Flags that change the bytes are honoured:
+// -minencodethreads= / -maxencodethreads= / -evensplit (thread-segment selection), -rejectprogressive / -allowprogressive,
+// and -zlib0: a restored JPEG is written as a zlib stream of stored blocks (jpgcoder.cc:2089, 2200-2220), default name
+// <stem>.jpg.z (open_fdout, jpgcoder.cc:1477-1479).  A .lep whose magic is CE B6 (zeta) is always restored that way; the
+// JPEG -> .lep direction ignores -zlib0.
 //
 // Batch mode (no reference counterpart; a GPU wants thousands of files per call, the reference one per process):
 //   lepton-b200 -outdir=DIR [-devices=0,1,...] a.jpg b.lep c.jpg ...
 // every positional argument is an input, the direction is chosen per file, all JPEGs go through ONE
 // lepb200_compress_jpegs call and all .lep files through ONE lepb200_decompress_leps call; outputs are DIR/<name>.lep /
-// DIR/<name>.jpg.  With -devices= the files are dealt to one codec per GPU, balanced by bytes (lepb200_*_multi).  A file that fails reports its ExitCode on stderr and does not stop the others; the exit status is
+// DIR/<name>.jpg (DIR/<name>.jpg.z for zlib0 output).  With -devices= the files are dealt to one codec per GPU, balanced by bytes (lepb200_*_multi).  A file that fails reports its ExitCode on stderr and does not stop the others; the exit status is
 // the first non-zero one.
 #include <cstdio>
 #include <cstdlib>
@@ -43,8 +46,10 @@ static std::string base_name(const std::string& path) {
 }
 
 // -outdir=DIR: all inputs in two library calls (one per direction)
-static int run_batch(const std::vector<std::string>& files, const std::string& outdir, const std::vector<int>& devices, int allow_progressive, int min_threads, int max_threads, int even_split, int verify) {
-    struct Item { std::string name; std::vector<uint8_t> data; bool is_jpeg = false; int status = 0; };
+static bool is_lep_magic(const std::vector<uint8_t>& d) { return (d[0] == 0xCF && d[1] == 0x84) || (d[0] == 0xCE && d[1] == 0xB6); }
+
+static int run_batch(const std::vector<std::string>& files, const std::string& outdir, const std::vector<int>& devices, int allow_progressive, int min_threads, int max_threads, int even_split, int verify, int zlib0) {
+    struct Item { std::string name; std::vector<uint8_t> data; bool is_jpeg = false, zeta = false; int status = 0; };
     std::vector<Item> items(files.size());
     int first_err = 0;
     for (size_t i = 0; i < files.size(); ++i) {
@@ -59,7 +64,8 @@ static int run_batch(const std::vector<std::string>& files, const std::string& o
         }
         if (!it.status) {
             it.is_jpeg = it.data[0] == 0xFF && it.data[1] == 0xD8;
-            if (!it.is_jpeg && !(it.data[0] == 0xCF && it.data[1] == 0x84)) it.status = 42;          // UNSUPPORTED_JPEG
+            it.zeta = it.data[0] == 0xCE && it.data[1] == 0xB6;
+            if (!it.is_jpeg && !is_lep_magic(it.data)) it.status = 42;                              // UNSUPPORTED_JPEG
         }
     }
     // one codec per GPU; the host threads are divided between them
@@ -75,6 +81,7 @@ static int run_batch(const std::vector<std::string>& files, const std::string& o
         lepb200_codec_set_encode_threads(c, min_threads, max_threads);
         lepb200_codec_set_even_split(c, even_split);
         lepb200_codec_set_verify(c, verify);
+        lepb200_codec_set_zlib0(c, zlib0);
         codecs.push_back(c);
     }
     for (int dir = 0; dir < 2; ++dir) {                      // 0: JPEG -> .lep, 1: .lep -> JPEG
@@ -95,7 +102,7 @@ static int run_batch(const std::vector<std::string>& files, const std::string& o
             Item& it = items[idx[k]];
             it.status = res[k].status == LEPB200_ST_NOT_HANDLED ? 42 : res[k].status;
             if (it.status) continue;
-            const std::string out = outdir + "/" + base_name(it.name) + (dir == 0 ? ".lep" : ".jpg");
+            const std::string out = outdir + "/" + base_name(it.name) + (dir == 0 ? ".lep" : (zlib0 || it.zeta) ? ".jpg.z" : ".jpg");
             FILE* fo = fopen(out.c_str(), "wb");
             if (!fo || fwrite(res[k].data, 1, res[k].len, fo) != res[k].len) it.status = 33;
             if (fo) fclose(fo);
@@ -119,6 +126,7 @@ int main(int argc, char** argv) {
     int verify = 1;              // the reference verifies every file it writes unless told -skipverify (jpgcoder.cc:107-112, 1095-1110)
     int min_threads = 1, max_threads = 8;   // -minencodethreads= / -maxencodethreads=: bounds of the thread-segment count (change the .lep bytes)
     int allow_progressive = 1;   // this build follows the reference compiled with DEFAULT_ALLOW_PROGRESSIVE (CMakeLists.txt:293)
+    int zlib0 = 0;               // -zlib0: restored JPEGs are written as zlib streams
     for (int i = 1; i < argc; ++i) {
         const char* a = argv[i];
         if (a[0] == '-' && a[1] != 0) {
@@ -135,10 +143,11 @@ int main(int argc, char** argv) {
             if (!strcmp(a, "-verify") || !strcmp(a, "-verification") || !strcmp(a, "-roundtrip") || !strcmp(a, "-validate") ||
                 !strcmp(a, "-validation")) { verify = 1; continue; }
             if (!strcmp(a, "-rejectprogressive")) { allow_progressive = 0; continue; }
+            if (!strcmp(a, "-zlib0")) { zlib0 = 1; continue; }
             if (!strcmp(a, "-allowprogressive") || !strcmp(a, "-forceprogressive")) { allow_progressive = 1; continue; }
             if (!strcmp(a, "-socket") || !strncmp(a, "-socket=", 8) || !strncmp(a, "-listen", 7) || !strcmp(a, "-fork") ||
                 !strcmp(a, "-benchmark") || !strcmp(a, "-lepcat") || !strncmp(a, "-startbyte", 10) || !strncmp(a, "-trunc=", 7) ||
-                !strcmp(a, "-ujg") || !strcmp(a, "-brotliheader") || !strncmp(a, "-embedding", 10) || !strcmp(a, "-zlib0") || !strcmp(a, "-ans")) {
+                !strcmp(a, "-ujg") || !strcmp(a, "-brotliheader") || !strncmp(a, "-embedding", 10) || !strcmp(a, "-ans")) {
                 fprintf(stderr, "lepton-b200: option %s is outside this build\n", a);
                 return 13;   // VERSION_UNSUPPORTED
             }
@@ -152,14 +161,15 @@ int main(int argc, char** argv) {
         return 1;
     }
     if (devices.empty()) devices.push_back(device);
-    if (!outdir.empty()) return run_batch(files, outdir, devices, allow_progressive, min_threads, max_threads, even_split, verify);
+    if (!outdir.empty()) return run_batch(files, outdir, devices, allow_progressive, min_threads, max_threads, even_split, verify, zlib0);
     std::vector<uint8_t> in;
     FILE* fi = files[0] == "-" ? stdin : fopen(files[0].c_str(), "rb");
     if (!fi) { fprintf(stderr, "lepton-b200: cannot open %s\n", files[0].c_str()); return 9; }   // FILE_NOT_FOUND
     if (!read_all(fi, in)) return 33;                                                            // OS_ERROR
     if (fi != stdin) fclose(fi);
     if (in.size() < 2) return 3;                                                                 // SHORT_READ
-    const bool is_jpeg = in[0] == 0xFF && in[1] == 0xD8, is_lep = in[0] == 0xCF && in[1] == 0x84;
+    const bool is_jpeg = in[0] == 0xFF && in[1] == 0xD8, is_lep = is_lep_magic(in);
+    const bool zlib_out = is_lep && (zlib0 || (in[0] == 0xCE && in[1] == 0xB6));
     if (!is_jpeg && !is_lep) { fprintf(stderr, "lepton-b200: input is neither JPEG nor Lepton\n"); return 42; }
     std::string outname;
     if (files.size() > 1) outname = files[1];
@@ -168,7 +178,7 @@ int main(int argc, char** argv) {
         outname = files[0];
         size_t dot = outname.rfind('.');
         if (dot != std::string::npos) outname.resize(dot);
-        outname += is_jpeg ? ".lep" : ".jpg";
+        outname += is_jpeg ? ".lep" : zlib_out ? ".jpg.z" : ".jpg";
     }
     lepb200_codec* codec = nullptr;
     int rc = lepb200_codec_create(&codec, device, 0);
@@ -177,6 +187,7 @@ int main(int argc, char** argv) {
     lepb200_codec_set_encode_threads(codec, min_threads, max_threads);
     lepb200_codec_set_even_split(codec, even_split);
     lepb200_codec_set_verify(codec, verify);
+    lepb200_codec_set_zlib0(codec, zlib0);
     lepb200_buffer ib = {in.data(), in.size()};
     lepb200_result res = {nullptr, 0, 0};
     rc = is_jpeg ? lepb200_compress_jpegs(codec, &ib, 1, &res) : lepb200_decompress_leps(codec, &ib, 1, &res);
