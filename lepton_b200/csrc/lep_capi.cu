@@ -20,24 +20,12 @@
 #include "lep_huffpar.cu"
 #include "lep_huffenc.cu"
 #include "lep_mux.cu"
+#include "lep_plan.cuh"
 #include "lep_host.h"
 
 using namespace lepb200;
 
 namespace {
-
-// zig-zag position of each raster index (reference src/vp8/model/jpeg_meta.hh:13-23)
-const uint8_t k_zigzag[64] = {
-    0, 1, 5, 6, 14, 15, 27, 28, 2, 4, 7, 13, 16, 26, 29, 42, 3, 8, 12, 17, 25, 30, 41, 43, 9, 11, 18, 24, 31, 40, 44, 53,
-    10, 19, 23, 32, 39, 45, 52, 54, 20, 22, 33, 38, 46, 51, 55, 60, 21, 34, 37, 47, 50, 56, 59, 61, 35, 36, 48, 49, 57, 58, 62, 63};
-// first column of icos_base_8192_scaled (src/vp8/model/jpeg_meta.hh:48-58): entries [i*8]
-const int k_icos_base_col0[8] = {8192, 11363, 10703, 9633, 8192, 6436, 4433, 2260};
-// src/vp8/model/model.hh:264-274
-const uint16_t k_freqmax[64] = {
-    1024, 931, 985, 968, 1020, 968, 1020, 1020, 932, 858, 884, 840, 932, 838, 854, 854,
-    985, 884, 871, 875, 985, 878, 871, 854, 967, 841, 876, 844, 967, 886, 870, 837,
-    1020, 932, 985, 967, 1020, 969, 1020, 1020, 969, 838, 878, 886, 969, 838, 969, 838,
-    1020, 854, 871, 870, 1010, 969, 1020, 1020, 1020, 854, 854, 838, 1020, 838, 1020, 838};
 
 struct DevBuf {
     void* p = nullptr;
@@ -52,6 +40,10 @@ struct DevBuf {
         return e;
     }
     void release() { if (p) cudaFree(p); p = nullptr; cap = 0; }
+    DevBuf() = default;
+    DevBuf(const DevBuf&) = delete;
+    DevBuf& operator=(const DevBuf&) = delete;
+    ~DevBuf() { release(); }
 };
 struct HostBuf {
     void* p = nullptr;
@@ -66,9 +58,11 @@ struct HostBuf {
         return e;
     }
     void release() { if (p) cudaFreeHost(p); p = nullptr; cap = 0; }
+    HostBuf() = default;
+    HostBuf(const HostBuf&) = delete;
+    HostBuf& operator=(const HostBuf&) = delete;
+    ~HostBuf() { release(); }
 };
-
-inline size_t align_up(size_t v, size_t a) { return (v + a - 1) / a * a; }
 
 }  // namespace
 
@@ -87,10 +81,7 @@ struct lepb200_ctx {
     HostBuf h_henc_out, h_henc_segs, h_henc_desc;
     cudaEvent_t status_ev = nullptr;       // parts mode: the D2H of the decode batch's segment records, queued ahead of the part copies
     bool status_queued = false;
-    std::vector<size_t> henc_off;         // per image: offset of its scan bytes in the output buffers (SIZE_MAX = skipped)
-    std::vector<int> henc_seg_first;      // per image: index of its first segment record
-    std::vector<int> henc_seg_count;      // per image: its number of segment records
-    int henc_nseg = 0;
+    HuffEncodePlan henc;                  // jobs of the last Huffman encode (henc.off: where each image's scan bytes lie in the output buffers)
     // parts of the last lepb200_huffman_encode_resident_parts call: image range, segment range, byte range of the output,
     // the event behind the part's D2H copies on copy_stream
     struct HEncPart { int i0, i1, s0, s1; size_t b0, b1; cudaEvent_t done; };
@@ -100,12 +91,9 @@ struct lepb200_ctx {
     HostBuf h_segs, h_dense, h_stage, h_hjobs, h_hpar;
     size_t resident_plane_total = 0;
     int resident_images = 0;
-    std::vector<ImageDesc> images;
-    std::vector<SegDesc> segs;
-    std::vector<int> order;
-    std::vector<size_t> seg_blocks;
-    std::vector<size_t> plane_bytes;      // per image*3
-    size_t row_stride = 0;
+    BatchPlan batch;                      // job tables of the current coder batch, device addresses once uploaded
+    HuffDecodePlan hdec;                  // jobs of the last Huffman decode
+    std::vector<int> rc_redo;             // serial range coder: segments it codes again
     int grid = 0;
     bool have_batch = false, launched = false, symbolised = false, is_encode = true;
     float last_ms = -1.f, last_ms_a = -1.f, last_ms_huff = -1.f;
@@ -135,8 +123,6 @@ struct lepb200_ctx {
     int dec_lanes = 4;                    // group kernel: lanes per thread-segment, 32 / dec_lanes segments per warp in lock step
     int dec_group_grid = 0;               // group kernel: CTAs of the current batch
     int dec_threads = 0;                  // group kernel: model slots of the current batch (0: the batch uses the warp kernel)
-    bool tokens_known = false;            // token streams laid out on the host from caller-supplied bounds (no counting pre-pass)
-    unsigned long long token_total = 0;
     bool stage_preuploaded = false;       // the caller pushed the staged scans itself (lepb200_huffman_stage_upload)
 };
 
@@ -150,61 +136,6 @@ struct lepb200_ctx {
     } while (0)
 
 namespace {
-
-// ProbabilityTablesBase::set_quantization_table (src/vp8/model/model.hh:247-290)
-int fill_quant(ImageDesc& d, int c, const uint16_t zz[64], bool check_zero) {
-    uint16_t* q = d.q[c];
-    for (int i = 0; i < 64; ++i) q[i] = zz[k_zigzag[i]];
-    for (int r = 0; r < 8; ++r) {
-        for (int i = 0; i < 8; ++i) {
-            d.icos_x[c][r * 8 + i] = k_icos_base_col0[i] * (int)q[i * 8 + r];
-            d.icos_y[c][r * 8 + i] = k_icos_base_col0[i] * (int)q[r * 8 + i];
-        }
-        if (d.icos_x[c][r * 8] == 0 || d.icos_y[c][r * 8] == 0) {
-            if (check_zero) return LEPB200_ST_UNSUPPORTED_JPEG_WITH_ZERO_IDCT_0;
-            // decode side (filetype == LEPTON, model.hh:257): the reference goes on and would divide by zero; refuse.
-            return LEPB200_ST_UNSUPPORTED_JPEG_WITH_ZERO_IDCT_0;
-        }
-    }
-    for (int k = 0; k < 64; ++k) {
-        uint16_t fm = (uint16_t)(k_freqmax[k] + q[k] - 1);
-        if (q[k]) fm = (uint16_t)(fm / q[k]);
-        int len = 0;
-        for (uint32_t v = fm; v; v >>= 1) ++len;
-        d.min_thr[c][k] = (uint8_t)(len > 7 ? len - 7 : 0);
-    }
-    return 0;
-}
-
-// Rows of component c coded by a segment [min_y, max_y) (row iteration of lepton_codec.hh:41-100).
-size_t segment_blocks(const lepb200_image& im, int min_y, int max_y, bool last) {
-    size_t n = 0;
-    int v0 = im.bcv[0] / im.mcuv;
-    for (int c = 0; c < im.ncmp; ++c) {
-        int mult = im.bcv[c] / im.mcuv;
-        long y0 = (long)(min_y / std::max(v0, 1)) * mult, y1 = last ? im.trunc_bcv[c] : (long)((max_y + v0 - 1) / std::max(v0, 1)) * mult;
-        y1 = std::min<long>(y1, im.trunc_bcv[c]);
-        if (y1 > y0) n += (size_t)(y1 - y0) * im.bch[c];
-    }
-    return n;
-}
-
-int validate_image(lepb200_ctx* ctx, const lepb200_image& im) {
-    if (im.ncmp < 1 || im.ncmp > 3 || im.mcuv <= 0 || im.nseg < 1 || im.nseg > LEPB200_MAX_SEGMENTS) {
-        ctx->err = "invalid image descriptor (ncmp/mcuv/nseg)";
-        return LEPB200_ERR_INVALID;
-    }
-    for (int c = 0; c < im.ncmp; ++c) {
-        if (im.bch[c] <= 0 || im.bcv[c] <= 0 || im.bcv[c] % im.mcuv || im.trunc_bcv[c] < 0 || im.trunc_bcv[c] > im.bcv[c] ||
-            im.trunc_bc[c] < 0 || (long long)im.trunc_bc[c] > (long long)im.bch[c] * im.bcv[c] || !im.planes[c]) {
-            ctx->err = "invalid component geometry";
-            return LEPB200_ERR_INVALID;
-        }
-    }
-    for (int s = 0; s + 1 < im.nseg; ++s)
-        if (im.luma_y_start[s] > im.luma_y_start[s + 1]) { ctx->err = "segment starts must be non-decreasing"; return LEPB200_ERR_INVALID; }
-    return 0;
-}
 
 // lep_decode_g2_kernel<G>: launch shape (warps per CTA, thread-segments per warp) and resident CTAs per SM
 template <int G> int group_ctas_per_sm() {
@@ -225,76 +156,12 @@ template <int G> void launch_group_kernel(int grid, cudaStream_t st, const Image
     lep_decode_g2_kernel<G><<<grid, G2Cfg<G>::THREADS, 0, st>>>(images, segs, first, count, order, counter, models, rows, row_stride);
 }
 
-// Common part of encode/decode upload: job tables, pools, plane arena layout.
+// Common part of encode/decode upload: job tables (lep_plan.cuh), launch shape, pools, upload of the tables.
 int build_batch(lepb200_ctx* ctx, const lepb200_image* images, int nimages, bool encode, const lepb200_stream* in) {
     ctx->have_batch = false; ctx->launched = false; ctx->is_encode = encode;
-    if (nimages <= 0 || !images) { ctx->err = "empty batch"; return LEPB200_ERR_INVALID; }
-    ctx->images.assign(nimages, ImageDesc());
-    ctx->segs.clear(); ctx->seg_blocks.clear(); ctx->plane_bytes.assign((size_t)nimages * 3, 0);
-    size_t plane_total = 0, stream_total = 0, row_stride = 0;
-    unsigned long long token_total = 0;   // token arena layout when every segment comes with a caller-supplied bound
-    bool tokens_known = encode;
-    int sidx = 0;
-    for (int i = 0; i < nimages; ++i) {
-        const lepb200_image& im = images[i];
-        int v = validate_image(ctx, im);
-        if (v) return v;
-        ImageDesc& d = ctx->images[i];
-        memset(&d, 0, sizeof(d));
-        d.ncmp = im.ncmp; d.mcuv = im.mcuv;
-        int qstatus = 0;
-        size_t rs = 0;
-        for (int c = 0; c < im.ncmp; ++c) {
-            d.bch[c] = im.bch[c]; d.bcv[c] = im.bcv[c]; d.trunc_bcv[c] = im.trunc_bcv[c]; d.trunc_bc[c] = im.trunc_bc[c];
-            d.mult[c] = im.bcv[c] / im.mcuv;
-            int qs = fill_quant(d, c, im.qtable_zigzag[c], encode);
-            if (qs) qstatus = qs;
-            size_t pb = (size_t)im.bch[c] * im.bcv[c] * 128;
-            ctx->plane_bytes[(size_t)i * 3 + c] = pb;
-            d.plane[c] = plane_total;                     // offset for now; rebased below
-            plane_total += align_up(pb, 256);
-            rs += (size_t)im.bch[c] * 16 + align_up((size_t)im.bch[c], 16);
-        }
-        row_stride = std::max(row_stride, align_up(rs, 256));
-        for (int s = 0; s < im.nseg; ++s, ++sidx) {
-            SegDesc sd;
-            memset(&sd, 0, sizeof(sd));
-            sd.image = i;
-            sd.min_y = im.luma_y_start[s];
-            sd.is_last = s + 1 == im.nseg;
-            sd.max_y = sd.is_last ? im.bcv[0] : im.luma_y_start[s + 1];
-            sd.status = qstatus;
-            size_t nb = segment_blocks(im, sd.min_y, sd.max_y, sd.is_last);
-            ctx->seg_blocks.push_back(nb);
-            if (encode) {
-                // 64 B/block is > 1.5x what q=100 photos need.  Dense noise needs more (up to about 7/8 byte per decision):
-                // such a stream moves to the overflow arena, sized from the exact length (parallel range coder, see
-                // lep_digit_offsets_kernel) or from a proven bound when the serial coder codes the segment again
-                // (rerun_overflowed_serial).  No stream is ever cut short.
-                size_t cap = align_up(nb * 64 + 4096, 256);
-                sd.stream = stream_total; sd.cap = (uint32_t)cap;
-                stream_total += cap;
-                sd.tokens = 0; sd.tok_cap = 0;                    // assigned on the device by the counting pre-pass ...
-                if (im.seg_token_bound[s]) {                      // ... unless the caller knows a bound (GPU Huffman decoder)
-                    const unsigned long long tcap = ((unsigned long long)im.seg_token_bound[s] + 64 + 63) & ~63ull;
-                    sd.tok_cap = tcap > 0xffffff00ull ? 0xffffff00u : (uint32_t)tcap;
-                    sd.tokens = token_total;
-                    token_total += sd.tok_cap;
-                } else {
-                    tokens_known = false;
-                }
-            } else {
-                sd.stream = stream_total; sd.cap = (uint32_t)in[sidx].len;
-                stream_total += align_up((size_t)in[sidx].len + 16, 16);
-            }
-            ctx->segs.push_back(sd);
-        }
-    }
-    const int nseg = (int)ctx->segs.size();
-    // largest segments first (longest-processing-time-first on the persistent warps)
-    ctx->order.resize(nseg);
-    for (int i = 0; i < nseg; ++i) ctx->order[i] = i;
-    std::stable_sort(ctx->order.begin(), ctx->order.end(), [&](int a, int b) { return ctx->seg_blocks[a] > ctx->seg_blocks[b]; });
+    BatchPlan& b = ctx->batch;
+    if (const char* e = plan_batch(b, images, nimages, encode, in)) { ctx->err = e; return LEPB200_ERR_INVALID; }
+    const int nseg = (int)b.segs.size();
 
     // persistent grid: as many CTAs as can be resident, but no more warps than segments
     int per_sm = 0;
@@ -304,12 +171,9 @@ int build_batch(lepb200_ctx* ctx, const lepb200_image* images, int nimages, bool
     const int wpc = encode ? ENC_WARPS_PER_CTA : DEC_WARPS_PER_CTA;
     int grid = std::max(1, std::min(per_sm * ctx->sm_count, (nseg + wpc - 1) / wpc));
     ctx->grid = grid;
-    ctx->row_stride = row_stride;
-    ctx->tokens_known = tokens_known;
-    ctx->token_total = token_total;
 
-    CK(ctx->d_planes.reserve(plane_total));
-    CK(ctx->d_streams.reserve(stream_total + 256));
+    CK(ctx->d_planes.reserve(b.plane_total));
+    CK(ctx->d_streams.reserve(b.stream_total + 256));
     CK(ctx->d_images.reserve(sizeof(ImageDesc) * nimages));
     CK(ctx->d_segs.reserve(sizeof(SegDesc) * nseg));
     CK(ctx->d_order.reserve(sizeof(int) * nseg));
@@ -324,17 +188,17 @@ int build_batch(lepb200_ctx* ctx, const lepb200_image* images, int nimages, bool
         const int per_cta = warps * per_warp;
         ctx->dec_group_grid = std::max(1, std::min(gsm * ctx->sm_count, (ctx->dec_threads + per_cta - 1) / per_cta));
         CK(ctx->d_models.reserve((size_t)ctx->dec_threads * MODEL_BYTES));
-        CK(ctx->d_rows.reserve((size_t)ctx->dec_group_grid * per_cta * row_stride));
+        CK(ctx->d_rows.reserve((size_t)ctx->dec_group_grid * per_cta * b.row_stride));
     } else {
         CK(ctx->d_models.reserve((size_t)grid * wpc * MODEL_BYTES));
-        CK(ctx->d_rows.reserve((size_t)grid * wpc * row_stride));
+        CK(ctx->d_rows.reserve((size_t)grid * wpc * b.row_stride));
     }
-    for (int i = 0; i < nimages; ++i)
-        for (int c = 0; c < ctx->images[i].ncmp; ++c) ctx->images[i].plane[c] += (unsigned long long)(uintptr_t)ctx->d_planes.p;
-    for (auto& sd : ctx->segs) sd.stream += (unsigned long long)(uintptr_t)ctx->d_streams.p;
-    CK(cudaMemcpyAsync(ctx->d_images.p, ctx->images.data(), sizeof(ImageDesc) * nimages, cudaMemcpyHostToDevice, ctx->stream));
-    CK(cudaMemcpyAsync(ctx->d_segs.p, ctx->segs.data(), sizeof(SegDesc) * nseg, cudaMemcpyHostToDevice, ctx->stream));
-    CK(cudaMemcpyAsync(ctx->d_order.p, ctx->order.data(), sizeof(int) * nseg, cudaMemcpyHostToDevice, ctx->stream));
+    for (auto& d : b.images)
+        for (int c = 0; c < d.ncmp; ++c) d.plane[c] += (unsigned long long)(uintptr_t)ctx->d_planes.p;
+    for (auto& sd : b.segs) sd.stream += (unsigned long long)(uintptr_t)ctx->d_streams.p;
+    CK(cudaMemcpyAsync(ctx->d_images.p, b.images.data(), sizeof(ImageDesc) * nimages, cudaMemcpyHostToDevice, ctx->stream));
+    CK(cudaMemcpyAsync(ctx->d_segs.p, b.segs.data(), sizeof(SegDesc) * nseg, cudaMemcpyHostToDevice, ctx->stream));
+    CK(cudaMemcpyAsync(ctx->d_order.p, b.order.data(), sizeof(int) * nseg, cudaMemcpyHostToDevice, ctx->stream));
     return 0;
 }
 
@@ -413,9 +277,6 @@ void lepb200_destroy(lepb200_ctx* ctx) {
     if (!ctx) return;
     cudaSetDevice(ctx->device);
     cudaStreamSynchronize(ctx->stream);
-    for (DevBuf* b : {&ctx->d_henc_out, &ctx->d_henc_imgs, &ctx->d_henc_segs, &ctx->d_henc_tabs, &ctx->d_huff, &ctx->d_hjobs, &ctx->d_htabs, &ctx->d_hrows, &ctx->d_hpar, &ctx->d_planes, &ctx->d_streams, &ctx->d_tokens, &ctx->d_dense, &ctx->d_images, &ctx->d_segs, &ctx->d_order, &ctx->d_counter, &ctx->d_models, &ctx->d_rows, &ctx->d_rc_ck, &ctx->d_rc_digits, &ctx->d_rc_ovf, &ctx->d_rc_redo, &ctx->d_gather, &ctx->d_lit})
-        b->release();
-    for (HostBuf* b : {&ctx->h_segs, &ctx->h_dense, &ctx->h_stage, &ctx->h_hjobs, &ctx->h_hpar}) b->release();
     cudaEventDestroy(ctx->ev0);
     cudaEventDestroy(ctx->ev1);
     cudaEventDestroy(ctx->ev_mid);
@@ -423,7 +284,7 @@ void lepb200_destroy(lepb200_ctx* ctx) {
     if (ctx->status_ev) cudaEventDestroy(ctx->status_ev);
     if (ctx->copy_stream) cudaStreamDestroy(ctx->copy_stream);
     cudaStreamDestroy(ctx->stream);
-    delete ctx;
+    delete ctx;                           // the buffers free themselves
 }
 
 void lepb200_release_device_buffers(lepb200_ctx* ctx) {
@@ -431,7 +292,10 @@ void lepb200_release_device_buffers(lepb200_ctx* ctx) {
     cudaSetDevice(ctx->device);
     cudaStreamSynchronize(ctx->stream);
     cudaStreamSynchronize(ctx->copy_stream);
-    for (DevBuf* b : {&ctx->d_henc_out, &ctx->d_henc_imgs, &ctx->d_henc_segs, &ctx->d_henc_tabs, &ctx->d_huff, &ctx->d_hjobs, &ctx->d_htabs, &ctx->d_hrows, &ctx->d_hpar, &ctx->d_planes, &ctx->d_streams, &ctx->d_tokens, &ctx->d_dense, &ctx->d_images, &ctx->d_segs, &ctx->d_order, &ctx->d_counter, &ctx->d_models, &ctx->d_rows, &ctx->d_rc_ck, &ctx->d_rc_digits, &ctx->d_rc_ovf, &ctx->d_rc_redo, &ctx->d_gather, &ctx->d_lit})
+    for (DevBuf* b : {&ctx->d_planes, &ctx->d_streams, &ctx->d_tokens, &ctx->d_dense, &ctx->d_huff, &ctx->d_hjobs, &ctx->d_htabs, &ctx->d_hrows,
+                      &ctx->d_hpar, &ctx->d_images, &ctx->d_segs, &ctx->d_order, &ctx->d_counter, &ctx->d_models, &ctx->d_rows, &ctx->d_henc_out,
+                      &ctx->d_henc_imgs, &ctx->d_henc_segs, &ctx->d_henc_tabs, &ctx->d_gather, &ctx->d_lit, &ctx->d_rc_ck, &ctx->d_rc_digits,
+                      &ctx->d_rc_ovf, &ctx->d_rc_redo})
         b->release();
     ctx->have_batch = ctx->launched = false;
 }
@@ -477,19 +341,19 @@ int lepb200_encode_upload(lepb200_ctx* ctx, const lepb200_image* images, int nim
     if (r) return r;
     for (int i = 0; i < nimages; ++i)
         for (int c = 0; c < images[i].ncmp; ++c)
-            CK(cudaMemcpyAsync(reinterpret_cast<void*>(ctx->images[i].plane[c]), images[i].planes[c], ctx->plane_bytes[(size_t)i * 3 + c],
+            CK(cudaMemcpyAsync(reinterpret_cast<void*>(ctx->batch.images[i].plane[c]), images[i].planes[c], ctx->batch.plane_bytes[(size_t)i * 3 + c],
                                cudaMemcpyHostToDevice, ctx->stream));
     return encode_prepass(ctx);
 }
 
 static int encode_prepass(lepb200_ctx* ctx) {
-    if (ctx->tokens_known) {              // bounds came with the images (GPU Huffman decoder): nothing to count, nothing to wait for
-        CK(ctx->d_tokens.reserve((size_t)ctx->token_total * 2 + 256));
+    if (ctx->batch.tokens_known) {        // bounds came with the images (GPU Huffman decoder): nothing to count, nothing to wait for
+        CK(ctx->d_tokens.reserve((size_t)ctx->batch.token_total * 2 + 256));
         ctx->have_batch = true;
         return LEPB200_OK;
     }
     // pre-pass: per-segment token upper bounds -> exact-fit token arena (sizes depend on the data, so one sync here)
-    const int nseg = (int)ctx->segs.size();
+    const int nseg = (int)ctx->batch.segs.size();
     lep_count_kernel<<<nseg, CNT_THREADS, 0, ctx->stream>>>(static_cast<const ImageDesc*>(ctx->d_images.p), static_cast<SegDesc*>(ctx->d_segs.p), nseg);
     CK(cudaGetLastError());
     unsigned long long* d_total = reinterpret_cast<unsigned long long*>(static_cast<uint8_t*>(ctx->d_counter.p) + 64);
@@ -500,14 +364,12 @@ static int encode_prepass(lepb200_ctx* ctx) {
     CK(cudaMemcpyAsync(&total_tokens, d_total, sizeof(total_tokens), cudaMemcpyDeviceToHost, ctx->stream));
     CK(cudaStreamSynchronize(ctx->stream));
     CK(ctx->d_tokens.reserve((size_t)total_tokens * 2 + 256));
-    ctx->token_total = total_tokens;
+    ctx->batch.token_total = total_tokens;
     ctx->have_batch = true;
     return LEPB200_OK;
 }
 
 // ------------------------------------------------------------------------------------------------ GPU Huffman decode
-static bool build_table_dev(const lepb200_hufftable& in, HuffTableDev& t) { return huff_build_table(in.bits, in.vals, t); }
-
 uint8_t* lepb200_huffman_stage_reserve(lepb200_ctx* ctx, size_t bytes) {
     if (!ctx) return nullptr;
     if (cudaSetDevice(ctx->device) != cudaSuccess) return nullptr;
@@ -532,33 +394,6 @@ int lepb200_huffman_decode_to_device(lepb200_ctx* ctx, lepb200_jpeg_scan* scans,
     if (!ctx || !scans || n <= 0) return LEPB200_ERR_INVALID;
     CK(cudaSetDevice(ctx->device));
     ctx->have_batch = false; ctx->launched = false; ctx->resident_images = 0;
-    std::vector<HuffJob> jobs(n);
-    std::vector<HuffTableDev> tabs;
-    std::vector<std::pair<const lepb200_hufftable*, int>> seen;     // dedupe identical tables (most files share the standard ones)
-    std::vector<char> tab_ok;                                       // build result per table: a cache hit on a table that failed to build fails too
-    auto table_index = [&](const lepb200_hufftable& t, bool& ok) -> int {
-        for (auto& s : seen) if (!memcmp(s.first, &t, sizeof(t))) { if (!tab_ok[s.second]) ok = false; return s.second; }
-        HuffTableDev d;
-        const bool built = build_table_dev(t, d);
-        if (!built) ok = false;
-        tabs.push_back(d);
-        tab_ok.push_back(built ? 1 : 0);
-        seen.emplace_back(&t, (int)tabs.size() - 1);
-        return (int)tabs.size() - 1;
-    };
-    size_t plane_total = 0, huff_total = 0, rows_total = 0;
-    uint32_t sub_total = 0;
-    std::vector<uint32_t> sub_base((size_t)n + 1, 0);
-    // in-place mode: the caller de-stuffed straight into this context's pinned staging buffer
-    // (lepb200_huffman_stage_reserve), 16-byte aligned with >= 16 spare bytes after each scan -> no gather copy
-    const uint8_t* stage0 = static_cast<const uint8_t*>(ctx->h_stage.p);
-    int inside = 0, placeholders = 0;
-    for (int i = 0; i < n; ++i)
-        if (scans[i].entropy == nullptr) ++placeholders;
-        else if (stage0 && scans[i].entropy >= stage0 && scans[i].entropy + scans[i].nbytes + 16 <= stage0 + ctx->h_stage.cap) ++inside;
-    if (inside != 0 && inside != n - placeholders) { ctx->err = "huffman_decode_to_device: scans partly inside the staging buffer"; return LEPB200_ERR_INVALID; }
-    const bool in_place = inside > 0 && inside == n - placeholders;
-    for (int i = 0; i < n; ++i) if (in_place && scans[i].entropy && ((scans[i].entropy - stage0) & 15)) { ctx->err = "huffman_decode_to_device: staged scan not 16-byte aligned"; return LEPB200_ERR_INVALID; }
     // sub-sequence length of the many-threads-per-image kernels: longer sub-sequences need fewer synchronisation passes
     // (8192 bits: 3, 4096: 5, 2048: 9 on 1080p files), as long as the batch still gives every SM its 2048 threads
     int sub_bits = ctx->huff_sub_bits;
@@ -568,50 +403,24 @@ int lepb200_huffman_decode_to_device(lepb200_ctx* ctx, lepb200_jpeg_scan* scans,
         sub_bits = 2048;
         for (int cand : {16384, 8192, 4096}) if (bits / (uint64_t)cand >= (uint64_t)ctx->sm_count * 2048) { sub_bits = cand; break; }
     }
-    for (int i = 0; i < n; ++i) {
-        lepb200_jpeg_scan& sc = scans[i];
-        HuffJob& jb = jobs[i];
-        memset(&jb, 0, sizeof(jb));
-        const bool placeholder = sc.entropy == nullptr;
-        bool ok = sc.ncmp >= 1 && sc.ncmp <= 3 && sc.mcuh > 0 && sc.mcuv > 0 && (placeholder || sc.rows);
-        jb.ncmp = sc.ncmp; jb.mcuh = sc.mcuh; jb.mcuv = sc.mcuv; jb.rsti = sc.rsti; jb.nbytes = sc.nbytes;
-        for (int c = 0; ok && c < sc.ncmp; ++c) {
-            jb.H[c] = sc.H[c]; jb.V[c] = sc.V[c];
-            ok = ok && sc.H[c] >= 1 && sc.H[c] <= 2 && sc.V[c] >= 1 && sc.V[c] <= 2;
-            jb.bch[c] = sc.mcuh * sc.H[c]; jb.bcv[c] = sc.mcuv * sc.V[c];
-            jb.nch[c] = sc.nch[c]; jb.ncv[c] = sc.ncv[c];
-            if (!placeholder) { jb.dc_tab[c] = table_index(sc.dc[c], ok); jb.ac_tab[c] = table_index(sc.ac[c], ok); }
-            jb.plane[c] = plane_total;
-            plane_total += align_up((size_t)jb.bch[c] * jb.bcv[c] * 128, 256);
-        }
-        jb.status = ok ? (placeholder ? HUFF_JOB_SKIP : 0) : LEPB200_ST_NOT_HANDLED;
-        if (placeholder) {
-            jb.huff = 0; jb.nbytes = 0;
-        } else if (in_place) {
-            jb.huff = (size_t)(sc.entropy - stage0);
-            huff_total = std::max(huff_total, align_up((size_t)jb.huff + sc.nbytes + 16, 16));
-        } else {
-            jb.huff = huff_total;
-            huff_total += align_up((size_t)sc.nbytes + 16, 16);
-        }
-        jb.rows = rows_total;
-        rows_total += (size_t)(sc.mcuv + 1) * sizeof(HuffRow);
-        // interleaved scans without restart intervals and with enough data take the many-threads-per-image kernels
-        const uint64_t bits = (uint64_t)sc.nbytes * 8;
-        jb.sub_base = sub_total;
-        if (ctx->huff_par && jb.status == 0 && sc.ncmp > 1 && sc.rsti == 0 && bits >= 4ull * (uint64_t)sub_bits && bits < (1ull << 32))
-            jb.nsub = (uint32_t)((bits + (uint64_t)sub_bits - 1) / (uint64_t)sub_bits);
-        sub_total += jb.nsub;
-        sub_base[i] = jb.sub_base;
+    // in-place mode: the caller de-stuffed straight into this context's pinned staging buffer
+    // (lepb200_huffman_stage_reserve), 16-byte aligned with >= 16 spare bytes after each scan -> no gather copy
+    HuffDecodePlan& p = ctx->hdec;
+    if (const char* e = plan_huffman_decode(p, scans, n, ctx->huff_par != 0, sub_bits, static_cast<const uint8_t*>(ctx->h_stage.p), ctx->h_stage.cap)) {
+        ctx->err = e;
+        return LEPB200_ERR_INVALID;
     }
-    sub_base[n] = sub_total;
+    std::vector<HuffJob>& jobs = p.jobs;
+    const std::vector<HuffTableDev>& tabs = p.tabs.tabs;
+    const size_t plane_total = p.plane_total, huff_total = p.huff_total, rows_total = p.rows_total;
+    const uint32_t sub_total = p.sub_total;
     CK(ctx->d_planes.reserve(plane_total + 256));
     CK(ctx->d_huff.reserve(huff_total + 256));
     CK(ctx->d_hrows.reserve(rows_total + 256));
     CK(ctx->d_htabs.reserve(sizeof(HuffTableDev) * std::max<size_t>(1, tabs.size())));
-    if (!in_place) CK(ctx->h_stage.reserve(huff_total + 256));
+    if (!p.in_place) CK(ctx->h_stage.reserve(huff_total + 256));
     uint8_t* hs = static_cast<uint8_t*>(ctx->h_stage.p);
-    if (in_place) {
+    if (p.in_place) {
         if (!ctx->stage_preuploaded)          // (a caller that uploads itself has zeroed the 16 bytes behind each scan)
             for (int i = 0; i < n; ++i) if (scans[i].entropy) memset(hs + jobs[i].huff + scans[i].nbytes, 0, 16);   // the decoder reads whole words past the end
     } else {
@@ -632,20 +441,17 @@ int lepb200_huffman_decode_to_device(lepb200_ctx* ctx, lepb200_jpeg_scan* scans,
             for (auto& t : th) t.join();
         }
     }
-    for (int i = 0; i < n; ++i) {
-        HuffJob& jb = jobs[i];
+    const unsigned long long d_rows = (unsigned long long)(uintptr_t)ctx->d_hrows.p;
+    for (HuffJob& jb : jobs) {
         jb.huff += (unsigned long long)(uintptr_t)ctx->d_huff.p;
-        jb.rows += (unsigned long long)(uintptr_t)ctx->d_hrows.p;
+        jb.rows += d_rows;
         for (int c = 0; c < jb.ncmp; ++c) jb.plane[c] += (unsigned long long)(uintptr_t)ctx->d_planes.p;
     }
-    std::vector<int> perm(n);
-    for (int i = 0; i < n; ++i) perm[i] = i;          // one warp per image: no geometry grouping needed
-    const std::vector<HuffJob>& sorted = jobs;
     CK(ctx->d_hjobs.reserve(align_up(sizeof(HuffJob) * n, 256)));
     CK(cudaMemsetAsync(ctx->d_planes.p, 0, plane_total, ctx->stream));
-    if (!(in_place && ctx->stage_preuploaded)) CK(cudaMemcpyAsync(ctx->d_huff.p, hs, huff_total, cudaMemcpyHostToDevice, ctx->stream));
+    if (!(p.in_place && ctx->stage_preuploaded)) CK(cudaMemcpyAsync(ctx->d_huff.p, hs, huff_total, cudaMemcpyHostToDevice, ctx->stream));
     ctx->stage_preuploaded = false;
-    CK(cudaMemcpyAsync(ctx->d_hjobs.p, sorted.data(), sizeof(HuffJob) * n, cudaMemcpyHostToDevice, ctx->stream));
+    CK(cudaMemcpyAsync(ctx->d_hjobs.p, jobs.data(), sizeof(HuffJob) * n, cudaMemcpyHostToDevice, ctx->stream));
 
     if (!tabs.empty()) CK(cudaMemcpyAsync(ctx->d_htabs.p, tabs.data(), sizeof(HuffTableDev) * tabs.size(), cudaMemcpyHostToDevice, ctx->stream));
     CK(cudaEventRecord(ctx->ev0, ctx->stream));
@@ -664,7 +470,7 @@ int lepb200_huffman_decode_to_device(lepb200_ctx* ctx, lepb200_jpeg_scan* scans,
         CK(ctx->h_hpar.reserve(align_up(((size_t)n + 1) * 4, 256) + 256));
         uint32_t* h_base = static_cast<uint32_t*>(ctx->h_hpar.p);
         unsigned int* h_dirty = reinterpret_cast<unsigned int*>(static_cast<uint8_t*>(ctx->h_hpar.p) + align_up(((size_t)n + 1) * 4, 256));
-        memcpy(h_base, sub_base.data(), ((size_t)n + 1) * 4);
+        memcpy(h_base, p.sub_base.data(), ((size_t)n + 1) * 4);
         CK(cudaMemcpyAsync(hp + o_base, h_base, ((size_t)n + 1) * 4, cudaMemcpyHostToDevice, ctx->stream));
         HpArrays a;
         a.exit = reinterpret_cast<unsigned long long*>(hp + o_exit); a.cnt = reinterpret_cast<uint4*>(hp + o_cnt);
@@ -707,16 +513,7 @@ int lepb200_huffman_decode_to_device(lepb200_ctx* ctx, lepb200_jpeg_scan* scans,
     CK(cudaMemcpyAsync(hrows, ctx->d_hrows.p, rows_total, cudaMemcpyDeviceToHost, ctx->stream));
     CK(cudaStreamSynchronize(ctx->stream));
     cudaEventElapsedTime(&ctx->last_ms_huff, ctx->ev0, ctx->ev_mid);
-    for (int k = 0; k < n; ++k) {
-        const int i = perm[k];
-        scans[i].status = hj[k].status == HUFF_JOB_SKIP ? 0 : hj[k].status;
-        scans[i].padbit = hj[k].padbit;
-        scans[i].end_bitpos = hj[k].end_bitpos;
-        scans[i].nrows = hj[k].nrows;
-        const size_t off = (size_t)(jobs[i].rows - (unsigned long long)(uintptr_t)ctx->d_hrows.p);
-        static_assert(sizeof(HuffRow) == sizeof(lepb200_huffrow), "row record layout");
-        if (hj[k].nrows > 0) memcpy(scans[i].rows, hrows + off, sizeof(HuffRow) * (size_t)std::min(hj[k].nrows, scans[i].mcuv + 1));
-    }
+    huffman_decode_results(scans, n, hj, hrows, d_rows);
     ctx->resident_plane_total = plane_total;
     ctx->resident_images = n;
     return LEPB200_OK;
@@ -736,7 +533,7 @@ int lepb200_encode_upload_resident(lepb200_ctx* ctx, const lepb200_image* images
     for (int i = 0; i < nimages; ++i)
         for (int c = 0; c < images[i].ncmp && c < 3; ++c)
             if (images[i].planes[c])
-                CK(cudaMemcpyAsync(reinterpret_cast<void*>(ctx->images[i].plane[c]), images[i].planes[c], ctx->plane_bytes[(size_t)i * 3 + c],
+                CK(cudaMemcpyAsync(reinterpret_cast<void*>(ctx->batch.images[i].plane[c]), images[i].planes[c], ctx->batch.plane_bytes[(size_t)i * 3 + c],
                                    cudaMemcpyHostToDevice, ctx->stream));
     ctx->resident_images = 0;
     return encode_prepass(ctx);
@@ -745,12 +542,12 @@ int lepb200_encode_upload_resident(lepb200_ctx* ctx, const lepb200_image* images
 int lepb200_encode_launch_symbolise(lepb200_ctx* ctx) {
     if (!ctx || !ctx->have_batch || !ctx->is_encode) { if (ctx) ctx->err = "encode_launch without encode_upload"; return LEPB200_ERR_INVALID; }
     CK(cudaSetDevice(ctx->device));
-    const int nseg = (int)ctx->segs.size();
+    const int nseg = (int)ctx->batch.segs.size();
     CK(cudaMemsetAsync(ctx->d_counter.p, 0, sizeof(int), ctx->stream));
     CK(cudaEventRecord(ctx->ev0, ctx->stream));
     lep_encode_kernel<<<ctx->grid, ENC_WARPS_PER_CTA * 32, 0, ctx->stream>>>(
         static_cast<const ImageDesc*>(ctx->d_images.p), static_cast<SegDesc*>(ctx->d_segs.p), nseg, static_cast<const int*>(ctx->d_order.p),
-        static_cast<int*>(ctx->d_counter.p), static_cast<uint16_t*>(ctx->d_models.p), static_cast<uint8_t*>(ctx->d_rows.p), ctx->row_stride,
+        static_cast<int*>(ctx->d_counter.p), static_cast<uint16_t*>(ctx->d_models.p), static_cast<uint8_t*>(ctx->d_rows.p), ctx->batch.row_stride,
         static_cast<uint16_t*>(ctx->d_tokens.p));
     CK(cudaGetLastError());
     CK(cudaEventRecord(ctx->ev_mid, ctx->stream));
@@ -762,13 +559,13 @@ int lepb200_encode_launch_symbolise(lepb200_ctx* ctx) {
 int lepb200_encode_launch_rangecode(lepb200_ctx* ctx) {
     if (!ctx || !ctx->symbolised || !ctx->is_encode) { if (ctx) ctx->err = "encode_launch_rangecode without encode_launch_symbolise"; return LEPB200_ERR_INVALID; }
     CK(cudaSetDevice(ctx->device));
-    const int nseg = (int)ctx->segs.size();
+    const int nseg = (int)ctx->batch.segs.size();
     if (ctx->rc_mode == 1) {
         // range-only pass -> digit layout (one small D2H + sync: the arena size depends on the data) -> parallel pieces -> carries
         SegDesc* ds = static_cast<SegDesc*>(ctx->d_segs.p);
         const int* dord = static_cast<const int*>(ctx->d_order.p);
         const uint16_t* dtok = static_cast<const uint16_t*>(ctx->d_tokens.p);
-        CK(ctx->d_rc_ck.reserve((((size_t)ctx->token_total >> 10) + 2 * (size_t)nseg + 8) * sizeof(unsigned long long)));
+        CK(ctx->d_rc_ck.reserve(rc_checkpoints(ctx->batch.token_total, nseg) * sizeof(unsigned long long)));
         unsigned long long* dck = static_cast<unsigned long long*>(ctx->d_rc_ck.p);
         const bool trace = getenv("LEPB200_TRACE") != nullptr;           // per-kernel times on stderr (diagnostics; adds a sync)
         cudaEvent_t te[4] = {nullptr, nullptr, nullptr, nullptr};
@@ -822,30 +619,16 @@ int lepb200_encode_launch(lepb200_ctx* ctx) {
     return r ? r : lepb200_encode_launch_rangecode(ctx);
 }
 
-// Serial range coder (rc_mode 0): it learns a stream's length only by writing it, so a stream longer than its slot comes
-// back with ST_OUT_OVERFLOW (kernel A's token overflow, ntok > tok_cap, is the other source of that status and stays an
-// error).  Its tokens are still in the arena: lep_rangecode_kernel codes those segments again, alone, into the overflow
-// arena, with a capacity no stream can reach.  Bound: before every decision the range is normalised (>= 128), and the
-// sub-range kept is >= 1 (split >= 1, and split <= 1 + (range - 1) * 255 / 256 < range), so a decision shifts at most 7 bits;
-// with the marker bit and the 32 stop decisions a segment shifts T <= 7 (ntok + 33) bits, and writes at most
-// (T - 16) / 8 bytes plus the zero byte of the stop rule.  hs (the segment records, fetched) is updated in place.
-static size_t serial_stream_bound(uint32_t ntok) { return align_up((7ull * ((unsigned long long)ntok + 33) + 8) / 8 + 2, 256); }
+// Serial range coder (rc_mode 0): codes the segments whose stream outgrew its slot again, into the overflow arena
+// (plan_serial_rerun).  hs (the segment records, fetched) is updated in place.
 static int rerun_overflowed_serial(lepb200_ctx* ctx, SegDesc* hs, int nseg) {
     if (ctx->rc_mode == 1) return LEPB200_OK;
-    std::vector<int> redo;
-    size_t total = 0;
-    for (int s = 0; s < nseg; ++s)
-        if (hs[s].status == ST_OUT_OVERFLOW && hs[s].ntok <= hs[s].tok_cap) { redo.push_back(s); total += serial_stream_bound(hs[s].ntok); }
+    std::vector<int>& redo = ctx->rc_redo;
+    const size_t total = plan_serial_rerun(hs, nseg, redo);
     if (redo.empty()) return LEPB200_OK;
     CK(ctx->d_rc_ovf.reserve(total));
     CK(ctx->d_rc_redo.reserve(sizeof(int) * redo.size()));
-    size_t off = 0;
-    for (int s : redo) {
-        hs[s].stream = (unsigned long long)(uintptr_t)ctx->d_rc_ovf.p + off;
-        hs[s].cap = (uint32_t)serial_stream_bound(hs[s].ntok);
-        hs[s].status = ST_OK; hs[s].len = 0;
-        off += hs[s].cap;
-    }
+    for (int s : redo) hs[s].stream += (unsigned long long)(uintptr_t)ctx->d_rc_ovf.p;
     const int n = (int)redo.size();
     CK(cudaMemcpyAsync(ctx->d_segs.p, hs, sizeof(SegDesc) * nseg, cudaMemcpyHostToDevice, ctx->stream));
     CK(cudaMemcpyAsync(ctx->d_rc_redo.p, redo.data(), sizeof(int) * n, cudaMemcpyHostToDevice, ctx->stream));
@@ -861,7 +644,7 @@ static int rerun_overflowed_serial(lepb200_ctx* ctx, SegDesc* hs, int nseg) {
 int lepb200_encode_fetch(lepb200_ctx* ctx, lepb200_stream* out) {
     if (!ctx || !ctx->launched || !ctx->is_encode || !out) { if (ctx) ctx->err = "encode_fetch without encode_launch"; return LEPB200_ERR_INVALID; }
     CK(cudaSetDevice(ctx->device));
-    const int nseg = (int)ctx->segs.size();
+    const int nseg = (int)ctx->batch.segs.size();
     CK(ctx->h_segs.reserve(sizeof(SegDesc) * nseg + sizeof(unsigned long long) * nseg));
     SegDesc* hs = static_cast<SegDesc*>(ctx->h_segs.p);
     CK(cudaMemcpyAsync(hs, ctx->d_segs.p, sizeof(SegDesc) * nseg, cudaMemcpyDeviceToHost, ctx->stream));
@@ -876,7 +659,7 @@ int lepb200_encode_fetch(lepb200_ctx* ctx, lepb200_stream* out) {
         offs[s] = total;
         size_t n = hs[s].status == 0 ? hs[s].len : 0;
         total += align_up(n, 16);
-        alg += (uint64_t)ctx->seg_blocks[s] * 128 + n;
+        alg += (uint64_t)ctx->batch.seg_blocks[s] * 128 + n;
     }
     ctx->alg_bytes = alg;
     const size_t dense_bytes = align_up(total, 256);
@@ -906,7 +689,7 @@ int lepb200_encode_fetch(lepb200_ctx* ctx, lepb200_stream* out) {
 int lepb200_encode_fetch_files(lepb200_ctx* ctx, const lepb200_buffer* headers, lepb200_result* files) {
     if (!ctx || !ctx->launched || !ctx->is_encode || !headers || !files) { if (ctx) ctx->err = "encode_fetch_files without encode_launch"; return LEPB200_ERR_INVALID; }
     CK(cudaSetDevice(ctx->device));
-    const int nseg = (int)ctx->segs.size(), nimg = (int)ctx->images.size();
+    const int nseg = (int)ctx->batch.segs.size(), nimg = (int)ctx->batch.images.size();
     CK(ctx->h_segs.reserve(sizeof(SegDesc) * nseg));
     SegDesc* hs = static_cast<SegDesc*>(ctx->h_segs.p);
     CK(cudaMemcpyAsync(hs, ctx->d_segs.p, sizeof(SegDesc) * nseg, cudaMemcpyDeviceToHost, ctx->stream));
@@ -937,7 +720,7 @@ int lepb200_encode_fetch_files(lepb200_ctx* ctx, const lepb200_buffer* headers, 
         for (int s = s0; s < s1; ++s) {
             if (hs[s].status && !st) st = hs[s].status;
             if (s - s0 < LEPB200_MAX_SEGMENTS) lens[s - s0] = hs[s].len;
-            alg += (uint64_t)ctx->seg_blocks[s] * 128 + (hs[s].status == 0 ? hs[s].len : 0);
+            alg += (uint64_t)ctx->batch.seg_blocks[s] * 128 + (hs[s].status == 0 ? hs[s].len : 0);
         }
         files[i].data = nullptr; files[i].len = 0; files[i].status = st;
         if (st == 0 && (ns < 1 || ns > LEPB200_MAX_SEGMENTS || !headers[i].data || headers[i].len == 0)) files[i].status = st = LEPB200_ST_NOT_HANDLED;
@@ -980,87 +763,23 @@ int lepb200_encode_images(lepb200_ctx* ctx, const lepb200_image* images, int nim
 }
 
 // ------------------------------------------------------------------------------------------------ GPU Huffman encode
-static bool build_enc_table(const lepb200_hufftable& in, HEncTable& t) {
-    memset(&t, 0, sizeof(t));
-    int code = 0, k = 0;
-    for (int len = 1; len <= 16; ++len) {
-        for (int i = 0; i < in.bits[len]; ++i, ++k, ++code) {
-            if (k >= 256 || code >= (1 << len)) return false;        // over-subscribed table
-            t.code[in.vals[k]] = (uint16_t)code;
-            t.len[in.vals[k]] = (uint8_t)len;
-        }
-        if (code > (1 << len)) return false;
-        code <<= 1;
-    }
-    return true;
-}
-
 static int henc_launch(lepb200_ctx* ctx, lepb200_henc_image* imgs, int n, int nparts) {
     if (!ctx || !imgs || n <= 0) return LEPB200_ERR_INVALID;
     ctx->henc_parts.clear();
-    if (!ctx->launched || ctx->is_encode || n != (int)ctx->images.size()) { ctx->err = "huffman_encode_resident: needs the decode batch just launched on this context"; return LEPB200_ERR_INVALID; }
+    if (!ctx->launched || ctx->is_encode || n != (int)ctx->batch.images.size()) { ctx->err = "huffman_encode_resident: needs the decode batch just launched on this context"; return LEPB200_ERR_INVALID; }
     CK(cudaSetDevice(ctx->device));
-    std::vector<HEncImage> hi(n);
-    std::vector<HEncSeg> hs;
-    std::vector<HEncTable> tabs;
-    std::vector<const lepb200_hufftable*> seen;
-    std::vector<char> tab_ok;                     // build result per table (a cache hit on a table that failed to build fails too)
-    auto table_index = [&](const lepb200_hufftable& t, bool& ok) -> int {
-        for (size_t q = 0; q < seen.size(); ++q) if (!memcmp(seen[q], &t, sizeof(t))) { if (!tab_ok[q]) ok = false; return (int)q; }
-        HEncTable e;
-        const bool built = build_enc_table(t, e);
-        if (!built) ok = false;
-        tabs.push_back(e);
-        tab_ok.push_back(built ? 1 : 0);
-        seen.push_back(&t);
-        return (int)tabs.size() - 1;
-    };
-    ctx->henc_off.assign(n, SIZE_MAX);
-    ctx->henc_seg_first.assign(n, -1);
-    ctx->henc_seg_count.assign(n, 0);
-    size_t total = 0;
-    for (int i = 0; i < n; ++i) {
-        lepb200_henc_image& im = imgs[i];
-        im.data = nullptr; im.status = 0;
-        HEncImage& d = hi[i];
-        memset(&d, 0, sizeof(d));
-        if (im.scan_bytes == 0) continue;
-        const ImageDesc& g = ctx->images[i];
-        bool ok = im.nseg >= 1 && im.nseg <= LEPB200_MAX_SEGMENTS && g.ncmp >= 1 && g.ncmp <= 3;
-        d.ncmp = g.ncmp; d.mcuv = g.mcuv; d.rsti = im.rsti; d.padbit = im.padbit; d.scan_len = im.scan_bytes;
-        for (int c = 0; ok && c < g.ncmp; ++c) {
-            ok = im.H[c] >= 1 && im.H[c] <= 2 && im.V[c] >= 1 && im.V[c] <= 2 && g.bch[c] % im.H[c] == 0 && g.bcv[c] == g.mcuv * im.V[c];
-            d.H[c] = im.H[c]; d.V[c] = im.V[c]; d.bch[c] = g.bch[c]; d.plane[c] = g.plane[c];
-            if (ok) { d.dc_tab[c] = table_index(im.dc[c], ok); d.ac_tab[c] = table_index(im.ac[c], ok); }
-        }
-        if (ok) {
-            d.mcuh = g.bch[0] / im.H[0];
-            for (int c = 1; ok && c < g.ncmp; ++c) ok = g.bch[c] / im.H[c] == d.mcuh;
-        }
-        if (!ok) { im.status = LEPB200_ST_NOT_HANDLED; im.scan_bytes = 0; continue; }
-        ctx->henc_off[i] = total;
-        ctx->henc_seg_first[i] = (int)hs.size();
-        ctx->henc_seg_count[i] = im.nseg;
-        uint32_t off = 0;
-        for (int k = 0; k < im.nseg; ++k) {
-            HEncSeg sg;
-            memset(&sg, 0, sizeof(sg));
-            sg.image = i; sg.my0 = im.seg[k].mcu_row_start; sg.my1 = im.seg[k].mcu_row_end;
-            for (int c = 0; c < 3; ++c) sg.lastdc[c] = im.seg[k].last_dc[c];
-            sg.ov_bits = im.seg[k].overhang_bits; sg.ov_byte = im.seg[k].overhang_byte;
-            sg.out_off = off; sg.expect = im.seg[k].expect_bytes; sg.is_last = k + 1 == im.nseg;
-            off += im.seg[k].expect_bytes;
-            hs.push_back(sg);
-        }
-        total += align_up((size_t)im.scan_bytes + 16, 256);
-    }
-    ctx->henc_nseg = (int)hs.size();
+    HuffEncodePlan& p = ctx->henc;
+    plan_huffman_encode(p, imgs, n, ctx->batch.images.data());
+    std::vector<HEncImage>& hi = p.images;
+    const std::vector<HEncSeg>& hs = p.segs;
+    const std::vector<HEncTable>& tabs = p.tabs.tabs;
+    const size_t total = p.total;
     if (hs.empty()) return LEPB200_OK;
     CK(ctx->d_henc_out.reserve(total + 256));
     CK(ctx->d_henc_imgs.reserve(sizeof(HEncImage) * n));
     CK(ctx->d_henc_segs.reserve(sizeof(HEncSeg) * hs.size()));
     CK(ctx->d_henc_tabs.reserve(sizeof(HEncTable) * std::max<size_t>(1, tabs.size())));
-    for (int i = 0; i < n; ++i) if (ctx->henc_off[i] != SIZE_MAX) hi[i].out = (unsigned long long)(uintptr_t)ctx->d_henc_out.p + ctx->henc_off[i];
+    for (int i = 0; i < n; ++i) if (p.off[i] != SIZE_MAX) hi[i].out += (unsigned long long)(uintptr_t)ctx->d_henc_out.p;
     // the records travel from pinned memory: a copy from pageable memory of this size would hold the calling thread
     // until the stream has reached it, i.e. for the whole decode kernel queued in front
     {
@@ -1094,7 +813,7 @@ static int henc_launch(lepb200_ctx* ctx, lepb200_henc_image* imgs, int n, int np
     }
     // the decode batch's segment records first: they must not queue behind the part copies on the copy stream
     {
-        const int nseg_dec = (int)ctx->segs.size();
+        const int nseg_dec = (int)ctx->batch.segs.size();
         CK(ctx->h_segs.reserve(sizeof(SegDesc) * nseg_dec));
         if (!ctx->status_ev) CK(cudaEventCreateWithFlags(&ctx->status_ev, cudaEventDisableTiming));
         CK(cudaStreamWaitEvent(ctx->copy_stream, ctx->ev1, 0));
@@ -1107,16 +826,16 @@ static int henc_launch(lepb200_ctx* ctx, lepb200_henc_image* imgs, int n, int np
         const size_t want_end = k + 1 == nparts ? total : total / nparts * (k + 1);
         int i1 = i0;
         size_t bend = 0;
-        auto end_of = [&](int i) { return ctx->henc_off[i] == SIZE_MAX ? (size_t)0 : ctx->henc_off[i] + align_up((size_t)imgs[i].scan_bytes + 16, 256); };
+        auto end_of = [&](int i) { return p.off[i] == SIZE_MAX ? (size_t)0 : p.off[i] + align_up((size_t)imgs[i].scan_bytes + 16, 256); };
         while (i1 < n && (k + 1 == nparts || std::max(bend, end_of(i1)) <= want_end || i1 == i0)) { bend = std::max(bend, end_of(i1)); ++i1; }
         lepb200_ctx::HEncPart pt;
         pt.i0 = i0; pt.i1 = i1; pt.s0 = -1; pt.s1 = -1; pt.b0 = SIZE_MAX; pt.b1 = 0; pt.done = ctx->part_events[2 * k + 1];
         for (int i = i0; i < i1; ++i) {
-            if (ctx->henc_off[i] == SIZE_MAX) continue;
-            if (pt.s0 < 0) pt.s0 = ctx->henc_seg_first[i];
-            pt.s1 = ctx->henc_seg_first[i] + imgs[i].nseg;
-            pt.b0 = std::min(pt.b0, ctx->henc_off[i]);
-            pt.b1 = std::max(pt.b1, ctx->henc_off[i] + (size_t)imgs[i].scan_bytes);
+            if (p.off[i] == SIZE_MAX) continue;
+            if (pt.s0 < 0) pt.s0 = p.seg_first[i];
+            pt.s1 = p.seg_first[i] + imgs[i].nseg;
+            pt.b0 = std::min(pt.b0, p.off[i]);
+            pt.b1 = std::max(pt.b1, p.off[i] + (size_t)imgs[i].scan_bytes);
         }
         if (pt.s0 >= 0) {
             const int ns = pt.s1 - pt.s0;
@@ -1144,52 +863,53 @@ int lepb200_huffman_encode_resident_parts(lepb200_ctx* ctx, lepb200_henc_image* 
 
 int lepb200_huffman_encode_parts(const lepb200_ctx* ctx) { return ctx ? (int)ctx->henc_parts.size() : 0; }
 
+// data / status of images [i0, i1) from the fetched scan bytes and segment records
+static void henc_results(const lepb200_ctx* ctx, lepb200_henc_image* imgs, int i0, int i1) {
+    const HuffEncodePlan& p = ctx->henc;
+    const HEncSeg* hs = static_cast<const HEncSeg*>(ctx->h_henc_segs.p);
+    for (int i = i0; i < i1; ++i) {
+        if (p.off[i] == SIZE_MAX) continue;
+        imgs[i].data = static_cast<const uint8_t*>(ctx->h_henc_out.p) + p.off[i];
+        int st = 0;
+        for (int k = 0; k < p.seg_count[i]; ++k) if (hs[p.seg_first[i] + k].status) st = 1;
+        imgs[i].status = st;
+    }
+}
+
 int lepb200_huffman_encode_wait_part(lepb200_ctx* ctx, lepb200_henc_image* imgs, int n, int part, int* first, int* last) {
-    if (!ctx || !imgs || !first || !last || n != (int)ctx->henc_off.size() || part < 0 || part >= (int)ctx->henc_parts.size()) return LEPB200_ERR_INVALID;
+    if (!ctx || !imgs || !first || !last || n != (int)ctx->henc.off.size() || part < 0 || part >= (int)ctx->henc_parts.size()) return LEPB200_ERR_INVALID;
     CK(cudaSetDevice(ctx->device));
     const lepb200_ctx::HEncPart& pt = ctx->henc_parts[part];
     CK(cudaEventSynchronize(pt.done));
-    const HEncSeg* hs = static_cast<const HEncSeg*>(ctx->h_henc_segs.p);
-    for (int i = pt.i0; i < pt.i1; ++i) {
-        if (ctx->henc_off[i] == SIZE_MAX) continue;
-        imgs[i].data = static_cast<const uint8_t*>(ctx->h_henc_out.p) + ctx->henc_off[i];
-        int st = 0;
-        for (int k = 0; k < imgs[i].nseg; ++k) if (hs[ctx->henc_seg_first[i] + k].status) st = 1;
-        imgs[i].status = st;
-    }
+    henc_results(ctx, imgs, pt.i0, pt.i1);
     *first = pt.i0; *last = pt.i1;
     return LEPB200_OK;
 }
 
 int lepb200_huffman_encode_fetch(lepb200_ctx* ctx, lepb200_henc_image* imgs, int n) {
-    if (!ctx || !imgs || n != (int)ctx->henc_off.size()) return LEPB200_ERR_INVALID;
-    if (ctx->henc_nseg == 0) return LEPB200_OK;
+    if (!ctx || !imgs || n != (int)ctx->henc.off.size()) return LEPB200_ERR_INVALID;
+    const HuffEncodePlan& p = ctx->henc;
+    if (p.segs.empty()) return LEPB200_OK;
     CK(cudaSetDevice(ctx->device));
     size_t total = 0;
-    for (int i = 0; i < n; ++i) if (ctx->henc_off[i] != SIZE_MAX) total = std::max(total, ctx->henc_off[i] + imgs[i].scan_bytes);
+    for (int i = 0; i < n; ++i) if (p.off[i] != SIZE_MAX) total = std::max(total, p.off[i] + imgs[i].scan_bytes);
     CK(ctx->h_henc_out.reserve(total + 256));
-    CK(ctx->h_henc_segs.reserve(sizeof(HEncSeg) * ctx->henc_nseg));
+    CK(ctx->h_henc_segs.reserve(sizeof(HEncSeg) * p.segs.size()));
     CK(cudaMemcpyAsync(ctx->h_henc_out.p, ctx->d_henc_out.p, total, cudaMemcpyDeviceToHost, ctx->stream));
-    CK(cudaMemcpyAsync(ctx->h_henc_segs.p, ctx->d_henc_segs.p, sizeof(HEncSeg) * ctx->henc_nseg, cudaMemcpyDeviceToHost, ctx->stream));
+    CK(cudaMemcpyAsync(ctx->h_henc_segs.p, ctx->d_henc_segs.p, sizeof(HEncSeg) * p.segs.size(), cudaMemcpyDeviceToHost, ctx->stream));
     CK(cudaStreamSynchronize(ctx->stream));
-    const HEncSeg* hs = static_cast<const HEncSeg*>(ctx->h_henc_segs.p);
-    for (int i = 0; i < n; ++i) {
-        if (ctx->henc_off[i] == SIZE_MAX) continue;
-        imgs[i].data = static_cast<const uint8_t*>(ctx->h_henc_out.p) + ctx->henc_off[i];
-        int st = 0;
-        for (int k = 0; k < imgs[i].nseg; ++k) if (hs[ctx->henc_seg_first[i] + k].status) st = 1;
-        imgs[i].status = st;
-    }
+    henc_results(ctx, imgs, 0, n);
     return LEPB200_OK;
 }
 
 int lepb200_huffman_encode_adler32(lepb200_ctx* ctx, int first, int last, uint32_t* adler) {
-    if (!ctx || !adler || first < 0 || first > last || last > (int)ctx->henc_off.size()) return LEPB200_ERR_INVALID;
+    if (!ctx || !adler || first < 0 || first > last || last > (int)ctx->henc.off.size()) return LEPB200_ERR_INVALID;
+    const HuffEncodePlan& p = ctx->henc;
     const HEncSeg* hs = static_cast<const HEncSeg*>(ctx->h_henc_segs.p);
     for (int i = first; i < last; ++i) {
         uLong a = adler32(0L, Z_NULL, 0);
-        for (int k = 0; ctx->henc_off[i] != SIZE_MAX && k < ctx->henc_seg_count[i]; ++k) {     // segments lie back to back, in order
-            const HEncSeg& sg = hs[ctx->henc_seg_first[i] + k];
+        for (int k = 0; p.off[i] != SIZE_MAX && k < p.seg_count[i]; ++k) {     // segments lie back to back, in order
+            const HEncSeg& sg = hs[p.seg_first[i] + k];
             a = adler32_combine(a, sg.adler, (z_off_t)sg.produced);
         }
         adler[i] = (uint32_t)a;
@@ -1205,19 +925,16 @@ static int decode_upload_impl(lepb200_ctx* ctx, const lepb200_image* images, int
     ctx->d_tokens.release();              // the encoder's token arena (the largest buffer of that direction) is not needed on the way back
     int r = build_batch(ctx, images, nimages, false, in);
     if (r) return r;
-    const int nseg = (int)ctx->segs.size();
+    const int nseg = (int)ctx->batch.segs.size();
     // planes start zeroed: blocks outside the coded range (truncated images) stay zero like the reference's calloc.
     // Issued first: the device clears them while the host packs the streams.
-    size_t plane_total = 0;
-    for (int i = 0; i < nimages; ++i)
-        for (int c = 0; c < images[i].ncmp; ++c) plane_total = std::max(plane_total, (size_t)(ctx->images[i].plane[c] - (unsigned long long)(uintptr_t)ctx->d_planes.p) + ctx->plane_bytes[(size_t)i * 3 + c]);
-    CK(cudaMemsetAsync(ctx->d_planes.p, 0, plane_total, ctx->stream));
+    CK(cudaMemsetAsync(ctx->d_planes.p, 0, ctx->batch.plane_total, ctx->stream));
     // pack the streams into the pinned staging buffer (over a gigabyte for a 4096-image batch: a single-threaded copy
     // loop took longer than the H2D itself) in a few slices of consecutive segments; every slice is packed by the
     // context's host threads and its H2D copy runs while the next one is packed
     const unsigned long long base = (unsigned long long)(uintptr_t)ctx->d_streams.p;
     size_t total = 0;
-    for (int s = 0; s < nseg; ++s) total = std::max(total, (size_t)(ctx->segs[s].stream - base) + in[s].len);
+    for (int s = 0; s < nseg; ++s) total = std::max(total, (size_t)(ctx->batch.segs[s].stream - base) + in[s].len);
     CK(ctx->h_stage.reserve(total + 16));
     uint8_t* hs = static_cast<uint8_t*>(ctx->h_stage.p);
     const int nslices = total > (size_t(64) << 20) ? 8 : 1;
@@ -1226,11 +943,11 @@ static int decode_upload_impl(lepb200_ctx* ctx, const lepb200_image* images, int
         // segments are laid out in order, so a slice is a contiguous byte range of the staging buffer
         const size_t want_end = total / nslices * (k + 1);
         int s1 = s0;
-        while (s1 < nseg && (k + 1 == nslices || (size_t)(ctx->segs[s1].stream - base) < want_end)) ++s1;
+        while (s1 < nseg && (k + 1 == nslices || (size_t)(ctx->batch.segs[s1].stream - base) < want_end)) ++s1;
         const int nt = std::max(1, std::min(ctx->host_threads, s1 - s0));
         auto pack = [&](int t) {
             for (int s = s0 + t; s < s1; s += nt) {
-                uint8_t* dst = hs + (ctx->segs[s].stream - base);
+                uint8_t* dst = hs + (ctx->batch.segs[s].stream - base);
                 if (!spans) { if (in[s].len) memcpy(dst, in[s].data, in[s].len); continue; }
                 size_t room = in[s].len;                       // the pieces of a stream as they lie in the caller's file
                 for (uint32_t q = span_first[s]; q < span_first[s + 1] && room; ++q) {
@@ -1246,8 +963,8 @@ static int decode_upload_impl(lepb200_ctx* ctx, const lepb200_image* images, int
             for (int t = 0; t < nt; ++t) th.emplace_back(pack, t);
             for (auto& t : th) t.join();
         }
-        const size_t b0 = (size_t)(ctx->segs[s0].stream - base);
-        const size_t b1 = s1 < nseg ? (size_t)(ctx->segs[s1].stream - base) : total;
+        const size_t b0 = (size_t)(ctx->batch.segs[s0].stream - base);
+        const size_t b1 = s1 < nseg ? (size_t)(ctx->batch.segs[s1].stream - base) : total;
         if (b1 > b0) CK(cudaMemcpyAsync(static_cast<uint8_t*>(ctx->d_streams.p) + b0, hs + b0, b1 - b0, cudaMemcpyHostToDevice, ctx->stream));
         s0 = s1;
     }
@@ -1268,7 +985,7 @@ int lepb200_decode_upload_gather(lepb200_ctx* ctx, const lepb200_image* images, 
 int lepb200_decode_launch(lepb200_ctx* ctx) {
     if (!ctx || !ctx->have_batch || ctx->is_encode) { if (ctx) ctx->err = "decode_launch without decode_upload"; return LEPB200_ERR_INVALID; }
     CK(cudaSetDevice(ctx->device));
-    const int nseg = (int)ctx->segs.size();
+    const int nseg = (int)ctx->batch.segs.size();
     CK(cudaMemsetAsync(ctx->d_counter.p, 0, sizeof(int), ctx->stream));
     CK(cudaEventRecord(ctx->ev0, ctx->stream));
     if (ctx->dec_threads > 0) {
@@ -1289,9 +1006,9 @@ int lepb200_decode_launch(lepb200_ctx* ctx) {
             uint16_t* dm = static_cast<uint16_t*>(ctx->d_models.p);
             uint8_t* dr = static_cast<uint8_t*>(ctx->d_rows.p);
             switch (ctx->dec_lanes) {
-            case 8: launch_group_kernel<8>(grid, ctx->stream, di, ds, first, count, dord, dcnt, dm, dr, ctx->row_stride); break;
-            case 32: launch_group_kernel<32>(grid, ctx->stream, di, ds, first, count, dord, dcnt, dm, dr, ctx->row_stride); break;
-            default: launch_group_kernel<4>(grid, ctx->stream, di, ds, first, count, dord, dcnt, dm, dr, ctx->row_stride); break;
+            case 8: launch_group_kernel<8>(grid, ctx->stream, di, ds, first, count, dord, dcnt, dm, dr, ctx->batch.row_stride); break;
+            case 32: launch_group_kernel<32>(grid, ctx->stream, di, ds, first, count, dord, dcnt, dm, dr, ctx->batch.row_stride); break;
+            default: launch_group_kernel<4>(grid, ctx->stream, di, ds, first, count, dord, dcnt, dm, dr, ctx->batch.row_stride); break;
             }
             CK(cudaGetLastError());
             ctx->launches += 1;
@@ -1300,7 +1017,7 @@ int lepb200_decode_launch(lepb200_ctx* ctx) {
     } else {
         lep_decode_kernel<<<ctx->grid, DEC_WARPS_PER_CTA * 32, 0, ctx->stream>>>(
             static_cast<const ImageDesc*>(ctx->d_images.p), static_cast<SegDesc*>(ctx->d_segs.p), nseg, static_cast<const int*>(ctx->d_order.p),
-            static_cast<int*>(ctx->d_counter.p), static_cast<uint16_t*>(ctx->d_models.p), static_cast<uint8_t*>(ctx->d_rows.p), ctx->row_stride);
+            static_cast<int*>(ctx->d_counter.p), static_cast<uint16_t*>(ctx->d_models.p), static_cast<uint8_t*>(ctx->d_rows.p), ctx->batch.row_stride);
         CK(cudaGetLastError());
     }
     CK(cudaEventRecord(ctx->ev1, ctx->stream));
@@ -1312,23 +1029,23 @@ int lepb200_decode_launch(lepb200_ctx* ctx) {
 
 int lepb200_decode_fetch(lepb200_ctx* ctx, const lepb200_image* images, int nimages, int32_t* status_out) {
     if (!ctx || !ctx->launched || ctx->is_encode) { if (ctx) ctx->err = "decode_fetch without decode_launch"; return LEPB200_ERR_INVALID; }
-    if (nimages != (int)ctx->images.size()) { ctx->err = "decode_fetch: batch size mismatch"; return LEPB200_ERR_INVALID; }
+    if (nimages != (int)ctx->batch.images.size()) { ctx->err = "decode_fetch: batch size mismatch"; return LEPB200_ERR_INVALID; }
     CK(cudaSetDevice(ctx->device));
-    const int nseg = (int)ctx->segs.size();
+    const int nseg = (int)ctx->batch.segs.size();
     CK(ctx->h_segs.reserve(sizeof(SegDesc) * nseg));
     SegDesc* hs = static_cast<SegDesc*>(ctx->h_segs.p);
     CK(cudaMemcpyAsync(hs, ctx->d_segs.p, sizeof(SegDesc) * nseg, cudaMemcpyDeviceToHost, ctx->stream));
     for (int i = 0; i < nimages; ++i)
         for (int c = 0; c < images[i].ncmp; ++c)
             if (images[i].planes[c])        // NULL: the caller does not need this plane on the host (scan re-encoded on the device)
-                CK(cudaMemcpyAsync(images[i].planes[c], reinterpret_cast<const void*>(ctx->images[i].plane[c]), ctx->plane_bytes[(size_t)i * 3 + c],
+                CK(cudaMemcpyAsync(images[i].planes[c], reinterpret_cast<const void*>(ctx->batch.images[i].plane[c]), ctx->batch.plane_bytes[(size_t)i * 3 + c],
                                    cudaMemcpyDeviceToHost, ctx->stream));
     CK(cudaStreamSynchronize(ctx->stream));
     CK(cudaEventElapsedTime(&ctx->last_ms, ctx->ev0, ctx->ev1));
     uint64_t alg = 0;
     for (int s = 0; s < nseg; ++s) {
         if (status_out) status_out[s] = hs[s].status;
-        alg += (uint64_t)ctx->seg_blocks[s] * 128 + ctx->segs[s].cap;
+        alg += (uint64_t)ctx->batch.seg_blocks[s] * 128 + ctx->batch.segs[s].cap;
     }
     ctx->alg_bytes = alg;
     return LEPB200_OK;
@@ -1337,7 +1054,7 @@ int lepb200_decode_fetch(lepb200_ctx* ctx, const lepb200_image* images, int nima
 int lepb200_decode_fetch_status(lepb200_ctx* ctx, int32_t* status_out) {
     if (!ctx || !status_out || !ctx->launched || ctx->is_encode) { if (ctx) ctx->err = "decode_fetch_status without decode_launch"; return LEPB200_ERR_INVALID; }
     CK(cudaSetDevice(ctx->device));
-    const int nseg = (int)ctx->segs.size();
+    const int nseg = (int)ctx->batch.segs.size();
     CK(ctx->h_segs.reserve(sizeof(SegDesc) * nseg));
     SegDesc* hs = static_cast<SegDesc*>(ctx->h_segs.p);
     if (ctx->status_queued) {                                            // queued by lepb200_huffman_encode_resident_parts ahead of its copies

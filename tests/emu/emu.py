@@ -18,7 +18,7 @@ CSRC = os.path.join(ROOT, "lepton_b200", "csrc")
 OUT = os.path.join(HERE, "_build", "libemu_kernels.so")
 SOURCES = [os.path.join(HERE, "emu_kernels.cc"), os.path.join(HERE, "cuda_shim.h"), os.path.join(HERE, "fake", "cuda_runtime.h"),
            os.path.join(CSRC, "lep_encode.cu"), os.path.join(CSRC, "lep_decode.cu"), os.path.join(CSRC, "lep_decode_g2.cu"),
-           os.path.join(CSRC, "lep_huff.cu"), os.path.join(CSRC, "lep_huffpar.cu"), os.path.join(CSRC, "lep_mux.cu"), os.path.join(CSRC, "lep_huffenc.cu"), os.path.join(CSRC, "lep_common.cuh"), os.path.join(CSRC, "lep_predict.cuh"), os.path.join(ROOT, "include", "lepton_b200.h")]
+           os.path.join(CSRC, "lep_huff.cu"), os.path.join(CSRC, "lep_huffpar.cu"), os.path.join(CSRC, "lep_mux.cu"), os.path.join(CSRC, "lep_huffenc.cu"), os.path.join(CSRC, "lep_plan.cuh"), os.path.join(CSRC, "lep_common.cuh"), os.path.join(CSRC, "lep_predict.cuh"), os.path.join(ROOT, "include", "lepton_b200.h")]
 
 KERNEL_WARP = 0
 
@@ -296,18 +296,25 @@ def henc_job(host_lep):
     return job
 
 
-def huffman_encode(job, img):
-    """lep_huffencode_kernel on the emulator: scan bytes, per-segment (status, bytes produced).  img: CoefImage with the planes."""
+def huffman_encode_segments(job, img, reverse=False):
+    """lep_huffencode_kernel on the emulator -> (scan bytes, per segment (status, first byte, bytes produced, Adler-32)).
+    img: CoefImage with the planes; reverse runs CTAs and threads in reverse order."""
     assert job.scan_bytes > 0
     planes = [np.ascontiguousarray(p, dtype=np.int16) for p in img.planes]
     pp = (ctypes.c_void_p * 3)(*[p.ctypes.data for p in planes] + [None] * (3 - len(planes)))
     bch = (ctypes.c_int * 3)(*list(img.bch) + [0] * (3 - len(img.bch)))
+    bcv = (ctypes.c_int * 3)(*list(img.bcv) + [0] * (3 - len(img.bcv)))
     out = (ctypes.c_uint8 * job.scan_bytes)()
-    st = (ctypes.c_int32 * 16)()
-    prod = (ctypes.c_uint32 * 16)()
+    st, off, prod, ad = (ctypes.c_int32 * 16)(), (ctypes.c_uint32 * 16)(), (ctypes.c_uint32 * 16)(), (ctypes.c_uint32 * 16)()
     L = lib()
     L.emu_huffman_encode.restype = ctypes.c_int
-    rc = L.emu_huffman_encode(ctypes.byref(job), img.ncmp, img.mcuv, pp, bch, out, st, prod)
+    rc = L.emu_huffman_encode(ctypes.byref(job), img.ncmp, img.mcuv, pp, bch, bcv, int(bool(reverse)), out, st, off, prod, ad)
     if rc != 0:
         raise RuntimeError("emu_huffman_encode failed with %d" % rc)
-    return bytes(out), [(st[k], prod[k]) for k in range(job.nseg)]
+    return bytes(out), [(st[k], off[k], prod[k], ad[k]) for k in range(job.nseg)]
+
+
+def huffman_encode(job, img):
+    """lep_huffencode_kernel on the emulator: scan bytes, per-segment (status, bytes produced).  img: CoefImage with the planes."""
+    scan, segs = huffman_encode_segments(job, img)
+    return scan, [(st, prod) for st, _, prod, _ in segs]

@@ -1,9 +1,9 @@
 // emu_kernels.cc -- runs the coder kernels on the CPU under the warp emulator of cuda_shim.h (test infrastructure).
 //
-// The kernel sources are compiled as host C++; this file builds the same job descriptors lep_capi.cu's build_batch /
-// lepb200_decode_upload build for the device (ImageDesc, SegDesc, order, work counter, zeroed model and row pools, zeroed
-// planes) with host addresses in place of device addresses and launches the kernel with its device launch shape.
-// Entry points mirror lepb200_decode_images / lepb200_encode_images (include/lepton_b200.h).
+// The kernel sources are compiled as host C++, and the job descriptors come from the same planner as the library's
+// (lep_plan.cuh: ImageDesc / SegDesc, HuffJob, HEncImage / HEncSeg, arena offsets, launch order).  This file rebases the
+// planned offsets onto host vectors (poisoned where the device arena is not cleared), launches the kernels with their
+// device launch shapes and runs the host steps between launches.  Entry points mirror the C ABI (include/lepton_b200.h).
 #include <algorithm>
 #include <cstdlib>
 #include <vector>
@@ -15,44 +15,25 @@
 #include "../../lepton_b200/csrc/lep_huffpar.cu"
 #include "../../lepton_b200/csrc/lep_mux.cu"
 #include "../../lepton_b200/csrc/lep_huffenc.cu"
+#include "../../lepton_b200/csrc/lep_plan.cuh"
 #include "../../include/lepton_b200.h"
 
 using namespace lepb200;
 
 namespace {
 
-const uint8_t k_zigzag[64] = {
-    0, 1, 5, 6, 14, 15, 27, 28, 2, 4, 7, 13, 16, 26, 29, 42, 3, 8, 12, 17, 25, 30, 41, 43, 9, 11, 18, 24, 31, 40, 44, 53,
-    10, 19, 23, 32, 39, 45, 52, 54, 20, 22, 33, 38, 46, 51, 55, 60, 21, 34, 37, 47, 50, 56, 59, 61, 35, 36, 48, 49, 57, 58, 62, 63};
-const int k_icos_base_col0[8] = {8192, 11363, 10703, 9633, 8192, 6436, 4433, 2260};
-const uint16_t k_freqmax[64] = {
-    1024, 931, 985, 968, 1020, 968, 1020, 1020, 932, 858, 884, 840, 932, 838, 854, 854,
-    985, 884, 871, 875, 985, 878, 871, 854, 967, 841, 876, 844, 967, 886, 870, 837,
-    1020, 932, 985, 967, 1020, 969, 1020, 1020, 969, 838, 878, 886, 969, 838, 969, 838,
-    1020, 854, 871, 870, 1010, 969, 1020, 1020, 1020, 854, 854, 838, 1020, 838, 1020, 838};
-
-// ProbabilityTablesBase::set_quantization_table (src/vp8/model/model.hh:247-290), as fill_quant in lep_capi.cu
-int fill_quant(ImageDesc& d, int c, const uint16_t zz[64]) {
-    uint16_t* q = d.q[c];
-    for (int i = 0; i < 64; ++i) q[i] = zz[k_zigzag[i]];
-    for (int r = 0; r < 8; ++r) {
-        for (int i = 0; i < 8; ++i) {
-            d.icos_x[c][r * 8 + i] = k_icos_base_col0[i] * (int)q[i * 8 + r];
-            d.icos_y[c][r * 8 + i] = k_icos_base_col0[i] * (int)q[r * 8 + i];
-        }
-        if (d.icos_x[c][r * 8] == 0 || d.icos_y[c][r * 8] == 0) return LEPB200_ST_UNSUPPORTED_JPEG_WITH_ZERO_IDCT_0;
-    }
-    for (int k = 0; k < 64; ++k) {
-        uint16_t fm = (uint16_t)(k_freqmax[k] + q[k] - 1);
-        if (q[k]) fm = (uint16_t)(fm / q[k]);
-        int len = 0;
-        for (uint32_t v = fm; v; v >>= 1) ++len;
-        d.min_thr[c][k] = (uint8_t)(len > 7 ? len - 7 : 0);
-    }
-    return 0;
+// host arena: a vector of n bytes + 512 filled with `fill`, used from its first 256-byte aligned byte (like a device allocation)
+uint8_t* host_arena(std::vector<uint8_t>& v, size_t n, uint8_t fill) {
+    v.assign(n + 512, fill);
+    return reinterpret_cast<uint8_t*>(align_up((size_t)(uintptr_t)v.data(), 256));
 }
 
-size_t align_up(size_t v, size_t a) { return (v + a - 1) / a * a; }
+// plane and stream offsets of a batch plan -> addresses in the host arenas
+void rebase(BatchPlan& b, uint8_t* planes, uint8_t* streams) {
+    for (auto& d : b.images)
+        for (int c = 0; c < d.ncmp; ++c) d.plane[c] += (unsigned long long)(uintptr_t)planes;
+    for (auto& sd : b.segs) sd.stream += (unsigned long long)(uintptr_t)streams;
+}
 
 struct LaunchArgs {
     int kernel;
@@ -86,62 +67,19 @@ extern "C" int emu_decode_images(int kernel, int grid_cap, const lepb200_image* 
                                  int32_t* status_out, uint64_t* ndecisions_out) {
     const int gl = kernel % 100;
     const bool group = kernel / 100 == 2 && (gl == 1 || gl == 2 || gl == 4 || gl == 8 || gl == 16 || gl == 32);
-    if (nimages <= 0 || !images || !in || (kernel != 0 && !group)) return LEPB200_ERR_INVALID;
-    std::vector<ImageDesc> descs(nimages);
-    std::vector<SegDesc> segs;
-    std::vector<size_t> seg_blocks;
-    std::vector<std::vector<uint8_t>> padded;          // streams with the 16 readable bytes the device arena has behind them
-    size_t row_stride = 0;
-    for (int i = 0; i < nimages; ++i) {
-        const lepb200_image& im = images[i];
-        if (im.ncmp < 1 || im.ncmp > 3 || im.mcuv <= 0 || im.nseg < 1 || im.nseg > LEPB200_MAX_SEGMENTS) return LEPB200_ERR_INVALID;
-        ImageDesc& d = descs[i];
-        memset(&d, 0, sizeof(d));
-        d.ncmp = im.ncmp; d.mcuv = im.mcuv;
-        int qstatus = 0;
-        size_t rs = 0;
-        for (int c = 0; c < im.ncmp; ++c) {
-            d.bch[c] = im.bch[c]; d.bcv[c] = im.bcv[c]; d.trunc_bcv[c] = im.trunc_bcv[c]; d.trunc_bc[c] = im.trunc_bc[c];
-            d.mult[c] = im.bcv[c] / im.mcuv;
-            const int qs = fill_quant(d, c, im.qtable_zigzag[c]);
-            if (qs) qstatus = qs;
-            d.plane[c] = (unsigned long long)(uintptr_t)im.planes[c];
-            memset(im.planes[c], 0, (size_t)im.bch[c] * im.bcv[c] * 128);
-            rs += (size_t)im.bch[c] * 16 + align_up((size_t)im.bch[c], 16);
-        }
-        row_stride = std::max(row_stride, align_up(rs, 256));
-        for (int s = 0; s < im.nseg; ++s) {
-            SegDesc sd;
-            memset(&sd, 0, sizeof(sd));
-            sd.image = i;
-            sd.min_y = im.luma_y_start[s];
-            sd.is_last = s + 1 == im.nseg;
-            sd.max_y = sd.is_last ? im.bcv[0] : im.luma_y_start[s + 1];
-            sd.status = qstatus;
-            const lepb200_stream& st = in[segs.size()];
-            padded.emplace_back((size_t)st.len + 16, 0xA5);      // the device arena is not cleared: whatever is behind a stream must not matter
-            if (st.len) memcpy(padded.back().data(), st.data, (size_t)st.len);
-            sd.cap = (uint32_t)st.len;
-            size_t nb = 0;                                  // segment_blocks of lep_capi.cu: only the launch order depends on it
-            const int v0 = std::max(im.bcv[0] / im.mcuv, 1);
-            for (int c = 0; c < im.ncmp; ++c) {
-                const int mult = im.bcv[c] / im.mcuv;
-                long y0 = (long)(sd.min_y / v0) * mult, y1 = sd.is_last ? im.trunc_bcv[c] : (long)((sd.max_y + v0 - 1) / v0) * mult;
-                y1 = std::min<long>(y1, im.trunc_bcv[c]);
-                if (y1 > y0) nb += (size_t)(y1 - y0) * im.bch[c];
-            }
-            seg_blocks.push_back(nb);
-            segs.push_back(sd);
-        }
-    }
-    const int nseg = (int)segs.size();
-    for (int s = 0; s < nseg; ++s) segs[s].stream = (unsigned long long)(uintptr_t)padded[s].data();
-    std::vector<int> order(nseg);
-    for (int i = 0; i < nseg; ++i) order[i] = i;
-    std::stable_sort(order.begin(), order.end(), [&](int a, int b) { return seg_blocks[a] > seg_blocks[b]; });
-
+    if (!in || (kernel != 0 && !group)) return LEPB200_ERR_INVALID;
+    BatchPlan b;
+    if (plan_batch(b, images, nimages, false, in)) return LEPB200_ERR_INVALID;
+    const int nseg = (int)b.segs.size();
+    // planes start zeroed like the device arena; the stream arena is not cleared: whatever is behind a stream must not matter
+    std::vector<uint8_t> pv, sv;
+    uint8_t* pbase = host_arena(pv, b.plane_total, 0);
+    uint8_t* sbase = host_arena(sv, b.stream_total, 0xA5);
+    for (int s = 0; s < nseg; ++s) if (in[s].len) memcpy(sbase + b.segs[s].stream, in[s].data, (size_t)in[s].len);
+    rebase(b, pbase, sbase);
+    std::vector<SegDesc>& segs = b.segs;
     LaunchArgs a;
-    a.kernel = kernel; a.images = descs.data(); a.segs = segs.data(); a.nseg = nseg; a.order = order.data(); a.row_stride = row_stride;
+    a.kernel = kernel; a.images = b.images.data(); a.segs = segs.data(); a.nseg = nseg; a.order = b.order.data(); a.row_stride = b.row_stride;
     int counter = 0;
     a.counter = &counter;
     unsigned grid, block;
@@ -161,9 +99,12 @@ extern "C" int emu_decode_images(int kernel, int grid_cap, const lepb200_image* 
     }
     const size_t slots = kernel == 0 ? (size_t)grid * DEC_WARPS_PER_CTA : (size_t)nseg;
     std::vector<uint16_t> models(slots * M_TOTAL, kernel == 0 ? 0x5a5a : 0);       // thread / group kernels: zero fill before the launch; the warp kernel clears its own
-    std::vector<uint8_t> rows((group ? group_slots : slots) * row_stride, 0);
+    std::vector<uint8_t> rows((group ? group_slots : slots) * b.row_stride, 0);
     a.models = models.data(); a.rows = rows.data();
     emu::launch(grid, block, kernel_body, &a);
+    for (int i = 0; i < nimages; ++i)
+        for (int c = 0; c < images[i].ncmp; ++c)
+            memcpy(images[i].planes[c], reinterpret_cast<const void*>(b.images[i].plane[c]), b.plane_bytes[(size_t)i * 3 + c]);
     for (int s = 0; s < nseg; ++s) {
         if (status_out) status_out[s] = segs[s].status;
         if (ndecisions_out) ndecisions_out[s] = (uint64_t)segs[s].ndecisions_lo | ((uint64_t)segs[s].ndecisions_hi << 32);
@@ -196,13 +137,13 @@ void enc_body(void* p) {
 // Kernel B after kernel A, with the launch shapes and the host steps of lepb200_encode_launch_rangecode /
 // lepb200_encode_fetch (lep_capi.cu): kernel 0 / 2 = the parallel range coder (async / register token feed): range pass,
 // digit offsets (+ overflow slots: `ovf` receives the overflow arena), pieces, carries; kernel 1 = the serial coder, then
-// rerun_overflowed_serial for the segments whose stream outgrew the slot.  `total_tokens` = size of the token arena.
+// plan_serial_rerun for the segments whose stream outgrew the slot.  `total_tokens` = size of the token arena.
 void run_range_coder(int kernel, EncArgs& a, unsigned long long total_tokens, std::vector<uint8_t>& ovf) {
     const int nseg = a.nseg;
     std::vector<unsigned long long> ck;
     std::vector<uint32_t> digits;
     if (kernel == 0 || kernel == 2) {
-        ck.assign(((size_t)total_tokens >> 10) + 2 * (size_t)nseg + 8, 0);
+        ck.assign(rc_checkpoints(total_tokens, nseg), 0);
         a.ck = ck.data();
         a.stage = kernel == 0 ? 5 : 4; emu::launch((unsigned)((nseg + RCT_THREADS - 1) / RCT_THREADS), RCT_THREADS, enc_body, &a);
         unsigned long long totals[2] = {0, 0};
@@ -219,21 +160,11 @@ void run_range_coder(int kernel, EncArgs& a, unsigned long long total_tokens, st
         return;
     }
     a.stage = 3; emu::launch((unsigned)((nseg + RC_THREADS - 1) / RC_THREADS), RC_THREADS, enc_body, &a);
-    std::vector<int> redo;                       // rerun_overflowed_serial
-    size_t total = 0;
-    auto bound = [](uint32_t ntok) { return align_up((7ull * ((unsigned long long)ntok + 33) + 8) / 8 + 2, 256); };
-    for (int s = 0; s < nseg; ++s)
-        if (a.segs[s].status == ST_OUT_OVERFLOW && a.segs[s].ntok <= a.segs[s].tok_cap) { redo.push_back(s); total += bound(a.segs[s].ntok); }
+    std::vector<int> redo;
+    const size_t total = plan_serial_rerun(a.segs, nseg, redo);
     if (redo.empty()) return;
     ovf.assign(total + 256, 0xC3);
-    size_t off = 0;
-    for (int s : redo) {
-        SegDesc& sd = a.segs[s];
-        sd.stream = (unsigned long long)(uintptr_t)(ovf.data() + off);
-        sd.cap = (uint32_t)bound(sd.ntok);
-        sd.status = ST_OK; sd.len = 0;
-        off += sd.cap;
-    }
+    for (int s : redo) a.segs[s].stream += (unsigned long long)(uintptr_t)ovf.data();
     const int* order = a.order;
     a.order = redo.data(); a.nseg = (int)redo.size();
     a.stage = 3; emu::launch((unsigned)((redo.size() + RC_THREADS - 1) / RC_THREADS), RC_THREADS, enc_body, &a);
@@ -250,65 +181,27 @@ void run_range_coder(int kernel, EncArgs& a, unsigned long long total_tokens, st
 // sum(nseg) entries) receives the token bound of every segment (the count pre-pass's, or the caller's seg_token_bound).
 extern "C" int emu_encode_images(int kernel, int grid_cap, const lepb200_image* images, int nimages, lepb200_stream* out, uint8_t* arena, size_t arena_cap,
                                  uint32_t* tok_caps) {
-    if (nimages <= 0 || !images || !out || !arena) return LEPB200_ERR_INVALID;
-    std::vector<ImageDesc> descs(nimages);
-    std::vector<SegDesc> segs;
-    std::vector<size_t> seg_blocks;
-    size_t row_stride = 0, stream_total = 0;
-    for (int i = 0; i < nimages; ++i) {
-        const lepb200_image& im = images[i];
-        if (im.ncmp < 1 || im.ncmp > 3 || im.mcuv <= 0 || im.nseg < 1 || im.nseg > LEPB200_MAX_SEGMENTS) return LEPB200_ERR_INVALID;
-        ImageDesc& d = descs[i];
-        memset(&d, 0, sizeof(d));
-        d.ncmp = im.ncmp; d.mcuv = im.mcuv;
-        int qstatus = 0;
-        size_t rs = 0;
-        for (int c = 0; c < im.ncmp; ++c) {
-            d.bch[c] = im.bch[c]; d.bcv[c] = im.bcv[c]; d.trunc_bcv[c] = im.trunc_bcv[c]; d.trunc_bc[c] = im.trunc_bc[c];
-            d.mult[c] = im.bcv[c] / im.mcuv;
-            const int qs = fill_quant(d, c, im.qtable_zigzag[c]);
-            if (qs) qstatus = qs;
-            d.plane[c] = (unsigned long long)(uintptr_t)im.planes[c];
-            rs += (size_t)im.bch[c] * 16 + align_up((size_t)im.bch[c], 16);
-        }
-        row_stride = std::max(row_stride, align_up(rs, 256));
-        for (int s = 0; s < im.nseg; ++s) {
-            SegDesc sd;
-            memset(&sd, 0, sizeof(sd));
-            sd.image = i;
-            sd.min_y = im.luma_y_start[s];
-            sd.is_last = s + 1 == im.nseg;
-            sd.max_y = sd.is_last ? im.bcv[0] : im.luma_y_start[s + 1];
-            sd.status = qstatus;
-            size_t nb = 0;
-            const int v0 = std::max(im.bcv[0] / im.mcuv, 1);
-            for (int c = 0; c < im.ncmp; ++c) {
-                const int mult = im.bcv[c] / im.mcuv;
-                long y0 = (long)(sd.min_y / v0) * mult, y1 = sd.is_last ? im.trunc_bcv[c] : (long)((sd.max_y + v0 - 1) / v0) * mult;
-                y1 = std::min<long>(y1, im.trunc_bcv[c]);
-                if (y1 > y0) nb += (size_t)(y1 - y0) * im.bch[c];
-            }
-            seg_blocks.push_back(nb);
-            const size_t cap = align_up(nb * 64 + 4096, 256);
-            sd.stream = stream_total; sd.cap = (uint32_t)cap;
-            stream_total += cap;
-            segs.push_back(sd);
-        }
-    }
-    const int nseg = (int)segs.size();
-    std::vector<uint8_t> streams(stream_total + 256, 0);
-    for (auto& sd : segs) sd.stream += (unsigned long long)(uintptr_t)streams.data();
-    std::vector<int> order(nseg);
-    for (int i = 0; i < nseg; ++i) order[i] = i;
-    std::stable_sort(order.begin(), order.end(), [&](int a, int b) { return seg_blocks[a] > seg_blocks[b]; });
+    if (!out || !arena) return LEPB200_ERR_INVALID;
+    BatchPlan b;
+    if (plan_batch(b, images, nimages, true, nullptr)) return LEPB200_ERR_INVALID;
+    const int nseg = (int)b.segs.size();
+    std::vector<uint8_t> pv, sv;
+    uint8_t* pbase = host_arena(pv, b.plane_total, 0);
+    uint8_t* sbase = host_arena(sv, b.stream_total, 0);
+    for (int i = 0; i < nimages; ++i)
+        for (int c = 0; c < images[i].ncmp; ++c) memcpy(pbase + b.images[i].plane[c], images[i].planes[c], b.plane_bytes[(size_t)i * 3 + c]);
+    rebase(b, pbase, sbase);
+    std::vector<SegDesc>& segs = b.segs;
 
     EncArgs a;
-    a.images = descs.data(); a.segs = segs.data(); a.nseg = nseg; a.order = order.data(); a.row_stride = row_stride;
+    a.images = b.images.data(); a.segs = segs.data(); a.nseg = nseg; a.order = b.order.data(); a.row_stride = b.row_stride;
     int counter = 0;
-    unsigned long long total_tokens = 0;
+    unsigned long long total_tokens = b.token_total;
     a.counter = &counter; a.total = &total_tokens; a.models = nullptr; a.rows = nullptr; a.tokens = nullptr;
-    a.stage = 0; emu::launch((unsigned)nseg, CNT_THREADS, enc_body, &a);
-    a.stage = 1; emu::launch(1, 1024, enc_body, &a);
+    if (!b.tokens_known) {            // count pre-pass -> token offsets, unless every segment came with a bound
+        a.stage = 0; emu::launch((unsigned)nseg, CNT_THREADS, enc_body, &a);
+        a.stage = 1; emu::launch(1, 1024, enc_body, &a);
+    }
     std::vector<uint16_t> tokens((size_t)total_tokens + 128, 0);
     a.tokens = tokens.data();
     std::vector<uint16_t> models;
@@ -317,7 +210,7 @@ extern "C" int emu_encode_images(int kernel, int grid_cap, const lepb200_image* 
         unsigned grid = (unsigned)((nseg + ENC_WARPS_PER_CTA - 1) / ENC_WARPS_PER_CTA);
         if (grid_cap > 0) grid = std::min(grid, (unsigned)grid_cap);
         models.assign((size_t)grid * ENC_WARPS_PER_CTA * M_TOTAL, 0x5a5a);      // the kernel clears its own
-        rows.assign((size_t)grid * ENC_WARPS_PER_CTA * row_stride, 0);
+        rows.assign((size_t)grid * ENC_WARPS_PER_CTA * b.row_stride, 0);
         a.models = models.data(); a.rows = rows.data();
         a.stage = 2; emu::launch(grid, ENC_WARPS_PER_CTA * 32, enc_body, &a);
     }
@@ -366,7 +259,7 @@ extern "C" int emu_range_code(int kernel, int reverse, int nseg, const uint16_t*
         SegDesc& sd = segs[s];
         memset(&sd, 0, sizeof(sd));
         sd.ntok = ntok[s];
-        sd.tok_cap = (uint32_t)(((unsigned long long)ntok[s] + 64 + 63) & ~63ull);
+        sd.tok_cap = token_slot(ntok[s]);
         sd.tokens = total_tokens;
         total_tokens += sd.tok_cap;
         sd.cap = caps[s];
@@ -415,8 +308,8 @@ extern "C" int emu_range_code(int kernel, int reverse, int nseg, const uint16_t*
 }
 
 // ---- baseline Huffman decode: lep_huffdecode_kernel alone (mode 0) or the sub-sequence kernels of lep_huffpar.cu followed
-// by it (mode 1), with the job set-up and the iteration loop of lepb200_huffman_decode_to_device (lep_capi.cu).
-// planes[3 * i + c] = host plane of component c of scan i (zeroed by the caller); scans[i] outputs are filled like the
+// by it (mode 1), on the jobs of plan_huffman_decode (lep_plan.cuh), without a staging buffer.
+// planes[3 * i + c] = host plane of component c of scan i (receives the decoded plane); scans[i] outputs are filled like the
 // device call fills them.  info[0] = synchronisation iterations, info[1] = images the serial kernel had to redo.
 namespace {
 struct HuffArgs { HuffJob* jobs; int n; const HuffTableDev* tabs; int ntabs; HpArrays a; int iter; int last_iter; unsigned int* dirty; int which; };
@@ -430,47 +323,21 @@ void huff_body(void* p) {
 }  // namespace
 
 extern "C" int emu_huffman_decode(int mode, int sub_bits, int iter_cap, lepb200_jpeg_scan* scans, int n, int16_t** planes, int* info) {
-    std::vector<HuffJob> jobs(n);
-    std::vector<HuffTableDev> tabs;
-    std::vector<std::vector<HuffRow>> rows(n);
-    std::vector<uint32_t> sub_base((size_t)n + 1, 0);
-    uint32_t sub_total = 0;
-    auto table_index = [&](const lepb200_hufftable& t, bool& ok) -> int {
-        HuffTableDev d;
-        if (!huff_build_table(t.bits, t.vals, d)) ok = false;
-        for (size_t k = 0; k < tabs.size(); ++k) if (!memcmp(&tabs[k], &d, sizeof(d))) return (int)k;
-        tabs.push_back(d);
-        return (int)tabs.size() - 1;
-    };
-    std::vector<std::vector<uint8_t>> padded(n);
-    for (int i = 0; i < n; ++i) {
-        lepb200_jpeg_scan& sc = scans[i];
-        HuffJob& jb = jobs[i];
-        memset(&jb, 0, sizeof(jb));
-        bool ok = sc.ncmp >= 1 && sc.ncmp <= 3 && sc.mcuh > 0 && sc.mcuv > 0 && sc.entropy;
-        jb.ncmp = sc.ncmp; jb.mcuh = sc.mcuh; jb.mcuv = sc.mcuv; jb.rsti = sc.rsti; jb.nbytes = sc.nbytes;
-        for (int c = 0; ok && c < sc.ncmp; ++c) {
-            jb.H[c] = sc.H[c]; jb.V[c] = sc.V[c];
-            ok = ok && sc.H[c] >= 1 && sc.H[c] <= 2 && sc.V[c] >= 1 && sc.V[c] <= 2;
-            jb.bch[c] = sc.mcuh * sc.H[c]; jb.bcv[c] = sc.mcuv * sc.V[c];
-            jb.nch[c] = sc.nch[c]; jb.ncv[c] = sc.ncv[c];
-            jb.dc_tab[c] = table_index(sc.dc[c], ok); jb.ac_tab[c] = table_index(sc.ac[c], ok);
-            jb.plane[c] = (unsigned long long)(uintptr_t)planes[3 * i + c];
-        }
-        jb.status = ok ? 0 : LEPB200_ST_NOT_HANDLED;
-        padded[i].assign((size_t)sc.nbytes + 32, 0);                 // the kernels read whole words past the end
-        if (sc.entropy) memcpy(padded[i].data(), sc.entropy, sc.nbytes);
-        jb.huff = (unsigned long long)(uintptr_t)padded[i].data();
-        rows[i].assign((size_t)sc.mcuv + 1, HuffRow());
-        jb.rows = (unsigned long long)(uintptr_t)rows[i].data();
-        const uint64_t bits = (uint64_t)sc.nbytes * 8;
-        jb.sub_base = sub_total;
-        if (mode == 1 && jb.status == 0 && sc.ncmp > 1 && sc.rsti == 0 && bits >= 4ull * (uint64_t)sub_bits)
-            jb.nsub = (uint32_t)((bits + (uint64_t)sub_bits - 1) / (uint64_t)sub_bits);
-        sub_total += jb.nsub;
-        sub_base[i] = jb.sub_base;
+    HuffDecodePlan p;
+    if (plan_huffman_decode(p, scans, n, mode == 1, sub_bits, nullptr, 0)) return LEPB200_ERR_INVALID;
+    std::vector<HuffJob>& jobs = p.jobs;
+    std::vector<uint8_t> hv, rv, pv;
+    uint8_t* hbase = host_arena(hv, p.huff_total, 0);              // the scans with the zero bytes the kernels read past their ends
+    uint8_t* rbase = host_arena(rv, p.rows_total, 0);
+    uint8_t* pbase = host_arena(pv, p.plane_total, 0);
+    for (int i = 0; i < n; ++i) if (scans[i].entropy) memcpy(hbase + jobs[i].huff, scans[i].entropy, scans[i].nbytes);
+    for (HuffJob& jb : jobs) {
+        jb.huff += (unsigned long long)(uintptr_t)hbase;
+        jb.rows += (unsigned long long)(uintptr_t)rbase;
+        for (int c = 0; c < std::min(jb.ncmp, 3); ++c) jb.plane[c] += (unsigned long long)(uintptr_t)pbase;
     }
-    sub_base[n] = sub_total;
+    const std::vector<HuffTableDev>& tabs = p.tabs.tabs;
+    const uint32_t sub_total = p.sub_total;
     HuffArgs h;
     memset(&h, 0, sizeof(h));
     h.jobs = jobs.data(); h.n = n; h.tabs = tabs.data(); h.ntabs = (int)tabs.size();
@@ -481,7 +348,7 @@ extern "C" int emu_huffman_decode(int mode, int sub_bits, int iter_cap, lepb200_
     std::vector<unsigned int> dirty(iter_cap + 4, 0);
     if (sub_total > 0) {
         h.a.exit = ex.data(); h.a.epoch = epoch.data(); h.a.cnt = cnt.data(); h.a.tok = tok.data();
-        h.a.sub_base = sub_base.data(); h.a.total = sub_total; h.a.sub_bits = (uint32_t)sub_bits;
+        h.a.sub_base = p.sub_base.data(); h.a.total = sub_total; h.a.sub_bits = (uint32_t)sub_bits;
         h.dirty = dirty.data(); h.last_iter = iter_cap;
         const unsigned grid = (sub_total + HP_THREADS - 1) / HP_THREADS;
         h.which = 1;
@@ -498,13 +365,11 @@ extern "C" int emu_huffman_decode(int mode, int sub_bits, int iter_cap, lepb200_
     for (int i = 0; i < n; ++i) if (jobs[i].nsub && !(jobs[i].par_done && !jobs[i].par_redo)) ++redo;
     h.which = 0;
     emu::launch((n + 3) / 4, 4 * 32, huff_body, &h);
-    for (int i = 0; i < n; ++i) {
-        scans[i].status = jobs[i].status;
-        scans[i].padbit = jobs[i].padbit;
-        scans[i].end_bitpos = jobs[i].end_bitpos;
-        scans[i].nrows = jobs[i].nrows;
-        if (scans[i].rows && jobs[i].nrows > 0) memcpy(scans[i].rows, rows[i].data(), sizeof(HuffRow) * (size_t)std::min(jobs[i].nrows, scans[i].mcuv + 1));
-    }
+    huffman_decode_results(scans, n, jobs.data(), rbase, (unsigned long long)(uintptr_t)rbase);
+    for (int i = 0; i < n; ++i)
+        for (int c = 0; c < std::min(jobs[i].ncmp, 3); ++c)
+            if (planes[3 * i + c])
+                memcpy(planes[3 * i + c], reinterpret_cast<const void*>(jobs[i].plane[c]), (size_t)jobs[i].bch[c] * jobs[i].bcv[c] * 128);
     if (info) { info[0] = iters; info[1] = redo; }
     return 0;
 }
@@ -560,64 +425,41 @@ extern "C" int emu_mux_files(int nfiles, const uint8_t* const* hdr, const size_t
 }
 
 
-// ---- baseline Huffman ENCODE for the way back (lep_huffenc.cu): the job set-up of lepb200_huffman_encode_resident (henc_launch,
-// lep_capi.cu) with host addresses, one launch over all thread-segments.  planes[c] = coefficient plane of component c
-// (AlignedBlock layout), bch[c] = blocks per row; out receives im->scan_bytes bytes; seg_status[k] / seg_produced[k] what each
-// segment reported.
+// ---- baseline Huffman ENCODE for the way back (lep_huffenc.cu): the jobs of lepb200_huffman_encode_resident
+// (plan_huffman_encode) for one image whose planes lie in the caller's memory, one launch over all thread-segments.
+// planes[c] = coefficient plane of component c (AlignedBlock layout), bch[c] / bcv[c] = its blocks per row / rows; out
+// receives im->scan_bytes bytes.  reverse = 1 runs the launch's CTAs and threads in reverse order (emu::g_reverse).  Per
+// segment (each output optional): status, first byte it wrote, bytes produced, Adler-32 of those bytes.
 namespace {
 struct HEncArgs { const HEncImage* images; HEncSeg* segs; int nseg; const HEncTable* tables; };
 void henc_body(void* p) { const HEncArgs& a = *static_cast<const HEncArgs*>(p); lep_huffencode_kernel(a.images, a.segs, a.nseg, a.tables); }
-bool emu_build_enc_table(const lepb200_hufftable& in, HEncTable& t) {      // build_enc_table of lep_capi.cu (build_huffcodes, jpgcoder.cc:5508-5540)
-    memset(&t, 0, sizeof(t));
-    int code = 0, k = 0;
-    for (int len = 1; len <= 16; ++len) {
-        for (int i = 0; i < in.bits[len]; ++i, ++k, ++code) {
-            if (k >= 256 || code >= (1 << len)) return false;
-            t.code[in.vals[k]] = (uint16_t)code;
-            t.len[in.vals[k]] = (uint8_t)len;
-        }
-        if (code > (1 << len)) return false;
-        code <<= 1;
-    }
-    return true;
-}
 }  // namespace
 
-extern "C" int emu_huffman_encode(const lepb200_henc_image* im, int ncmp, int mcuv, const int16_t* const* planes, const int* bch,
-                                  uint8_t* out, int32_t* seg_status, uint32_t* seg_produced) {
-    if (!im || !planes || !bch || !out || im->scan_bytes == 0 || im->nseg < 1 || im->nseg > LEPB200_MAX_SEGMENTS) return LEPB200_ERR_INVALID;
-    HEncImage d;
-    memset(&d, 0, sizeof(d));
-    std::vector<HEncTable> tabs;
-    d.ncmp = ncmp; d.mcuv = mcuv; d.rsti = im->rsti; d.padbit = im->padbit; d.scan_len = im->scan_bytes;
-    for (int c = 0; c < ncmp; ++c) {
-        d.H[c] = im->H[c]; d.V[c] = im->V[c]; d.bch[c] = bch[c];
-        d.plane[c] = (unsigned long long)(uintptr_t)planes[c];
-        HEncTable t;
-        if (!emu_build_enc_table(im->dc[c], t)) return LEPB200_ERR_INVALID;
-        d.dc_tab[c] = (int)tabs.size(); tabs.push_back(t);
-        if (!emu_build_enc_table(im->ac[c], t)) return LEPB200_ERR_INVALID;
-        d.ac_tab[c] = (int)tabs.size(); tabs.push_back(t);
+extern "C" int emu_huffman_encode(const lepb200_henc_image* im, int ncmp, int mcuv, const int16_t* const* planes, const int* bch, const int* bcv,
+                                  int reverse, uint8_t* out, int32_t* seg_status, uint32_t* seg_off, uint32_t* seg_produced, uint32_t* seg_adler) {
+    if (!im || !planes || !bch || !bcv || !out || ncmp < 1 || ncmp > 3) return LEPB200_ERR_INVALID;
+    ImageDesc g;
+    memset(&g, 0, sizeof(g));
+    g.ncmp = ncmp; g.mcuv = mcuv;
+    for (int c = 0; c < ncmp; ++c) { g.bch[c] = bch[c]; g.bcv[c] = bcv[c]; g.plane[c] = (unsigned long long)(uintptr_t)planes[c]; }
+    lepb200_henc_image job = *im;
+    HuffEncodePlan p;
+    plan_huffman_encode(p, &job, 1, &g);
+    if (p.segs.empty()) return LEPB200_ERR_INVALID;                  // nothing to encode, or a job the kernel does not take
+    std::vector<uint8_t> ov;
+    uint8_t* obase = host_arena(ov, p.total, 0xA5);
+    p.images[0].out += (unsigned long long)(uintptr_t)obase;
+    HEncArgs a{p.images.data(), p.segs.data(), (int)p.segs.size(), p.tabs.tabs.data()};
+    emu::g_reverse = reverse != 0;
+    emu::launch((unsigned)((p.segs.size() + HENC_WARPS - 1) / HENC_WARPS), HENC_WARPS * 32, henc_body, &a);
+    emu::g_reverse = false;
+    memcpy(out, obase, job.scan_bytes);
+    for (size_t k = 0; k < p.segs.size(); ++k) {
+        const HEncSeg& sg = p.segs[k];
+        if (seg_status) seg_status[k] = sg.status;
+        if (seg_off) seg_off[k] = sg.out_off;
+        if (seg_produced) seg_produced[k] = sg.produced;
+        if (seg_adler) seg_adler[k] = sg.adler;
     }
-    d.mcuh = bch[0] / im->H[0];
-    std::vector<uint8_t> obuf((size_t)im->scan_bytes + 256 + 512, 0xA5);
-    uint8_t* obase = reinterpret_cast<uint8_t*>(align_up((size_t)(uintptr_t)obuf.data(), 256));
-    d.out = (unsigned long long)(uintptr_t)obase;
-    std::vector<HEncSeg> segs;
-    uint32_t off = 0;
-    for (int k = 0; k < im->nseg; ++k) {
-        HEncSeg sg;
-        memset(&sg, 0, sizeof(sg));
-        sg.image = 0; sg.my0 = im->seg[k].mcu_row_start; sg.my1 = im->seg[k].mcu_row_end;
-        for (int c = 0; c < 3; ++c) sg.lastdc[c] = im->seg[k].last_dc[c];
-        sg.ov_bits = im->seg[k].overhang_bits; sg.ov_byte = im->seg[k].overhang_byte;
-        sg.out_off = off; sg.expect = im->seg[k].expect_bytes; sg.is_last = k + 1 == im->nseg;
-        off += im->seg[k].expect_bytes;
-        segs.push_back(sg);
-    }
-    HEncArgs a{&d, segs.data(), (int)segs.size(), tabs.data()};
-    emu::launch((unsigned)((segs.size() + HENC_WARPS - 1) / HENC_WARPS), HENC_WARPS * 32, henc_body, &a);
-    memcpy(out, obase, im->scan_bytes);
-    for (int k = 0; k < im->nseg; ++k) { if (seg_status) seg_status[k] = segs[k].status; if (seg_produced) seg_produced[k] = segs[k].produced; }
     return 0;
 }

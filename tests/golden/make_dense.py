@@ -4,7 +4,7 @@ what the UNMODIFIED reference CLI makes of them.
 
 Photos need well under 64 bytes of range-coder stream per 8x8 block; noise coded at quality 100 needs up to about 90.
 Every segment of every file here has a reference stream longer than the stream slot a segment starts with in the library
-(align_up(64 * blocks + 4096, 256) bytes, build_batch in lep_capi.cu): the library has to grow the stream to code these
+(align_up(64 * blocks + 4096, 256) bytes, plan_batch in lep_plan.cuh): the library has to grow the stream to code these
 files at all.  The script asserts that and records the margin of each segment.
 
 Run where oracle/_ref/lepton exists (oracle/Makefile builds it from the reference tree):
@@ -95,7 +95,7 @@ def corpus():
 
 
 def segment_blocks(lf):
-    """Blocks of every thread-segment of a .lep, counted like segment_blocks of lep_capi.cu."""
+    """Blocks of every thread-segment of a .lep, counted like segment_blocks of lep_plan.cuh."""
     import lepfmt
     f = lf.frame
     tbcv, _ = lepfmt.truncation(lf)

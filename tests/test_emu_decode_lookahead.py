@@ -20,7 +20,7 @@ from helpers import oracle_decode_image, oracle_encode_image, random_coef_image 
 GROUPS = [emu.KERNEL_G2(g) for g in (1, 2, 4, 8, 16, 32)]
 EDGE = list(range(50, 64))          # aligned indices of the 14 edge coefficients (raster 1..7, then 8, 16, .., 56)
 Q = 20                              # every quantiser: (freqmax + Q - 1) // Q <= (1024 + 19) // 20 = 52 < 128, so the
-                                    # min_threshold of every position (bit length - 7, lep_capi.cu fill_quant) is 0
+                                    # min_threshold of every position (bit length - 7, lep_plan.cuh fill_quant) is 0
 
 
 def with_quant(img, q):

@@ -35,7 +35,7 @@ def mult(e):
 
 def device_recode_gate(e):
     """Which files the device Huffman encoder takes (gpu_recode_setup in lep_recode.cc, then the geometry check of
-    henc_launch in lep_capi.cu): every colour file, and one-component files whose scan walks the whole plane (1x1
+    plan_huffman_encode in lep_plan.cuh): every colour file, and one-component files whose scan walks the whole plane (1x1
     sampling, no padding blocks).  The others go to the host re-encoder."""
     if len(e["sampling"]) == 3:
         return True

@@ -2,14 +2,11 @@
 thread-segment writes, on the CPU warp emulator (tests/emu); the stored-block framing of the host against the reference's
 -zlib0 output (tests/golden/zlib0.json, tests/golden/make_zlib0.py); and zeta-headed containers (magic CE B6) in the
 host .lep reader."""
-import ctypes
 import hashlib
 import os
-import subprocess
 import sys
 import zlib
 
-import numpy as np
 import pytest
 
 sys.path.insert(0, os.path.join(os.path.dirname(os.path.abspath(__file__)), "emu"))
@@ -20,34 +17,6 @@ from helpers import (DENSE, EXTREMES, GEOMETRY, GOLDEN, MANIFEST, dense_leps, ex
 from make_zlib0 import sweep_jpeg, zeta  # noqa: E402
 
 ZLIB0 = __import__("json").load(open(os.path.join(GOLDEN, "zlib0.json")))
-EMU_SRC = os.path.join(emu.HERE, "emu_zlib0.cc")
-EMU_OUT = os.path.join(emu.HERE, "_build", "libemu_zlib0.so")
-_LIB = None
-
-
-def emu_lib():
-    global _LIB
-    if _LIB is None:
-        srcs = emu.SOURCES + [EMU_SRC]
-        if not (os.path.exists(EMU_OUT) and all(os.path.getmtime(EMU_OUT) >= os.path.getmtime(s) for s in srcs)):
-            os.makedirs(os.path.dirname(EMU_OUT), exist_ok=True)
-            subprocess.check_call(["g++", "-O2", "-std=c++17", "-shared", "-fPIC", "-x", "c++", "-I", os.path.join(emu.HERE, "fake"),
-                                   "-Wno-unknown-pragmas", "-o", EMU_OUT, EMU_SRC])
-        _LIB = ctypes.CDLL(EMU_OUT)
-        _LIB.emu_huffman_encode_adler.restype = ctypes.c_int
-    return _LIB
-
-
-def huffman_encode_adler(job, img, reverse):
-    """lep_huffencode_kernel on the emulator -> (scan bytes, per segment (status, first byte, bytes produced, Adler-32))."""
-    planes = [np.ascontiguousarray(p, dtype=np.int16) for p in img.planes]
-    pp = (ctypes.c_void_p * 3)(*[p.ctypes.data for p in planes] + [None] * (3 - len(planes)))
-    bch = (ctypes.c_int * 3)(*list(img.bch) + [0] * (3 - len(img.bch)))
-    out = (ctypes.c_uint8 * job.scan_bytes)()
-    st, off, prod, ad = (ctypes.c_int32 * 16)(), (ctypes.c_uint32 * 16)(), (ctypes.c_uint32 * 16)(), (ctypes.c_uint32 * 16)()
-    rc = emu_lib().emu_huffman_encode_adler(ctypes.byref(job), img.ncmp, img.mcuv, pp, bch, int(bool(reverse)), out, st, off, prod, ad)
-    assert rc == 0
-    return bytes(out), [(st[k], off[k], prod[k], ad[k]) for k in range(job.nseg)]
 
 
 def adler32_combine(a, b, len_b):
@@ -98,7 +67,7 @@ def test_segment_adler32_of_the_encode_kernel(case, reverse):
     off, n = hl.scan_layout()
     job = emu.henc_job(hl)
     assert n > 0 and job.scan_bytes == n, name
-    scan, segs = huffman_encode_adler(job, HostJpeg(jpg).coef_image(), reverse)
+    scan, segs = emu.huffman_encode_segments(job, HostJpeg(jpg).coef_image(), reverse)
     assert scan == jpg[off:off + n], name
     assert [s[0] for s in segs] == [0] * job.nseg, (name, segs)
     pos, whole = 0, zlib.adler32(b"")
