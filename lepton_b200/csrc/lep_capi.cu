@@ -118,7 +118,7 @@ struct lepb200_ctx {
                                           // longer latency per chain -- it wins when the chains alone fill the machine (measured on an
                                           // H100 SXM at a 400 W limit, 1080p 4:2:0 images: 8192 segments 999 ms against 1339 ms,
                                           // 6144 segments 936 ms against 1035 ms; 4096 segments 850 ms against 722 ms)
-    int dec_threads_max = 16384;          // group kernel: segments per launch (one zero-filled 1.58 MB model each); more than a
+    int dec_threads_max = 16384;          // group kernel: segments per launch (one zero-filled 1.45 MB model each); more than a
                                           // decompress chunk of the file API holds, so that one launch covers a chunk
     int dec_lanes = 4;                    // group kernel: lanes per thread-segment, 32 / dec_lanes segments per warp in lock step
     int dec_group_grid = 0;               // group kernel: CTAs of the current batch
@@ -137,10 +137,14 @@ struct lepb200_ctx {
 
 namespace {
 
-// lep_decode_g2_kernel<G>: launch shape (warps per CTA, thread-segments per warp) and resident CTAs per SM
+// lep_decode_g2_kernel<G>: launch shape (warps per CTA, thread-segments per warp) and resident CTAs per SM.  The groups'
+// front regions take G2Cfg<G>::HOT_BYTES of dynamic shared memory (75 KB at G = 4: 32 groups of 2 400 bytes), more than the default 48 KB limit.
+template <int G> cudaError_t group_kernel_allow_smem() {
+    return cudaFuncSetAttribute(lep_decode_g2_kernel<G>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)G2Cfg<G>::HOT_BYTES);
+}
 template <int G> int group_ctas_per_sm() {
     int n = 0;
-    if (cudaOccupancyMaxActiveBlocksPerMultiprocessor(&n, lep_decode_g2_kernel<G>, G2Cfg<G>::THREADS, 0) != cudaSuccess) n = 1;
+    if (cudaOccupancyMaxActiveBlocksPerMultiprocessor(&n, lep_decode_g2_kernel<G>, G2Cfg<G>::THREADS, G2Cfg<G>::HOT_BYTES) != cudaSuccess) n = 1;
     return std::max(n, 1);
 }
 void group_launch_shape(int lanes, int& warps, int& per_warp, int& ctas_per_sm) {
@@ -153,7 +157,7 @@ void group_launch_shape(int lanes, int& warps, int& per_warp, int& ctas_per_sm) 
 }
 template <int G> void launch_group_kernel(int grid, cudaStream_t st, const ImageDesc* images, SegDesc* segs, int first, int count, const int* order,
                                           int* counter, uint16_t* models, uint8_t* rows, size_t row_stride) {
-    lep_decode_g2_kernel<G><<<grid, G2Cfg<G>::THREADS, 0, st>>>(images, segs, first, count, order, counter, models, rows, row_stride);
+    lep_decode_g2_kernel<G><<<grid, G2Cfg<G>::THREADS, G2Cfg<G>::HOT_BYTES, st>>>(images, segs, first, count, order, counter, models, rows, row_stride);
 }
 
 // Common part of encode/decode upload: job tables (lep_plan.cuh), launch shape, pools, upload of the tables.
@@ -248,7 +252,8 @@ int lepb200_create(lepb200_ctx** out, int device) {
         return LEPB200_ERR_CUDA;
     }
     if (cudaFuncSetAttribute(lep_rangepass_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)RCT_SMEM_BYTES) != cudaSuccess ||
-        cudaFuncSetAttribute(lep_rangepass_kernel<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)RCT_SMEM_TABLE_BYTES) != cudaSuccess) {
+        cudaFuncSetAttribute(lep_rangepass_kernel<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)RCT_SMEM_TABLE_BYTES) != cudaSuccess ||
+        group_kernel_allow_smem<4>() != cudaSuccess || group_kernel_allow_smem<8>() != cudaSuccess || group_kernel_allow_smem<32>() != cudaSuccess) {
         delete ctx;
         return LEPB200_ERR_CUDA;
     }

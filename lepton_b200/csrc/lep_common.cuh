@@ -40,35 +40,67 @@ constexpr unsigned FULL = 0xffffffffu;
 //     off the range coder's serial dependency chain;
 //   * the one state whose cached probability is not a function of its counts -- (1,255) reached through
 //     the "neverseen" overflow, p = 0 (branch.hh:87-90) -- is encoded with the otherwise unused low byte 0xff.
-// Exponent contexts are padded from 11 to 16 entries so that one context's unary chain is exactly one
-// 32-byte sector.  Only the bins the grammar can reach are allocated (10 of 26 nz-count bins).
+// Only the bins the grammar can reach are allocated (10 of 26 nz-count bins).
+//
+// Exponent chains are split.  Words k = 0..3 of a context take nearly all of its decisions on photographic input, so they
+// form a 4-word HEAD (8 bytes; the 12 bit-length contexts of one position fill 3 whole 32-byte sectors: the heads start on
+// a sector boundary and a position takes 96 bytes), and words k = 4..10 go to a
+// TAIL region of 8-word rows in the same context order.  All heads are one array (DC, 7x7, edge), so the word after head
+// word 3 is found from the address alone (m_exp_next).  The model starts with a FRONT region of small tables that nearly
+// every block reads -- signs, DC residuals, the fixed top rows of the 7x7 count trees, the DC exponent heads --
+// M_HOT words that the group decode kernel keeps in shared memory.
 // ------------------------------------------------------------------------------------------------------
-constexpr uint32_t M_NZ7 = 0;                                        // [2][10][6][32]
-constexpr uint32_t M_NZE = M_NZ7 + 2 * 10 * 6 * 32;                  // [2 kinds][2][8][8][3][4]  (kind 0 = 8x1 horizontal, 1 = 1x8 vertical)
+constexpr uint32_t M_SIGN = 0;                                       // [2][4][12]
+constexpr uint32_t M_RESDC = M_SIGN + 2 * 4 * 12;                    // [12][10]
+constexpr uint32_t M_NZ7T = M_RESDC + 12 * 10;                       // [2][10][8]: rows 3, 4, 5 of a 7x7 count tree (4 + 2 + 1 words, 1 pad)
+constexpr uint32_t M_EXPH = M_NZ7T + 2 * 10 * 8 + 8;                 // exponent heads [context][4] (8 words of padding before them):
+constexpr uint32_t M_EXPDC = M_EXPH;                                 //   [12][17]
+constexpr uint32_t M_HOT = M_EXPDC + 12 * 17 * 4;                    // end of the front region
+constexpr uint32_t M_EXP7 = M_HOT;                                   //   [2][10][49][12]
+constexpr uint32_t M_EXPX = M_EXP7 + 2 * 10 * 49 * 12 * 4;           //   [2][8][15][12]
+constexpr uint32_t M_EXPT = M_EXPX + 2 * 8 * 15 * 12 * 4;            // exponent tails [context][8]  (7 used)
+constexpr uint32_t M_NZ7 = M_EXPT + 2 * (M_EXPT - M_EXPH);           // [2][10][56]: rows 0, 1, 2 of a 7x7 count tree (32 + 16 + 8 words)
+constexpr uint32_t M_NZE = M_NZ7 + 2 * 10 * 56;                      // [2 kinds][2][8][8][3][4]  (kind 0 = 8x1 horizontal, 1 = 1x8 vertical)
 constexpr uint32_t M_RESN = M_NZE + 2 * 2 * 8 * 8 * 3 * 4;           // [2][64][10][16]  (10 used)
-constexpr uint32_t M_RESDC = M_RESN + 2 * 64 * 10 * 16;              // [12][16]
-constexpr uint32_t M_EXP7 = M_RESDC + 12 * 16;                       // [2][10][49][12][16]
-constexpr uint32_t M_EXPX = M_EXP7 + 2 * 10 * 49 * 12 * 16;          // [2][8][15][12][16]
-constexpr uint32_t M_EXPDC = M_EXPX + 2 * 8 * 15 * 12 * 16;          // [12][17][16]
-constexpr uint32_t M_SIGN = M_EXPDC + 12 * 17 * 16;                  // [2][4][12] (+pad)
-constexpr uint32_t M_THR = M_SIGN + 128;                             // [2][256][8][128]
+constexpr uint32_t M_THR = M_RESN + 2 * 64 * 10 * 16;                // [2][256][8][128]
 constexpr uint32_t M_TOTAL = M_THR + 2 * 256 * 8 * 128;              // u16 entries
 static_assert(M_TOTAL < (1u << 20), "branch index must fit in 20 bits");
-static_assert((M_TOTAL % 8) == 0, "model zero fill uses 16-byte stores");
+static_assert((M_TOTAL % 8) == 0 && (M_HOT % 8) == 0, "model zero fill uses 16-byte stores");
+static_assert((M_EXPH % 16) == 0 && (M_HOT % 16) == 0 && (M_EXPX % 16) == 0 && (M_TOTAL % 16) == 0,
+              "exponent heads start on a 32-byte sector in every model of a pool");
+static_assert((M_NZ7T % 8) == 0 && (M_NZ7 % 8) == 0 && (M_NZE % 4) == 0, "count tree rows are read as 8- and 16-byte vectors");
 constexpr size_t MODEL_BYTES = size_t(M_TOTAL) * 2;
 
-__host__ __device__ inline uint32_t m_nz7(int ci, int bin, int idx, int prefix) { return M_NZ7 + (((ci * 10 + bin) * 6 + idx) << 5) + prefix; }
-__host__ __device__ inline uint32_t m_nze(int vertical, int ci, int eob, int nzb, int idx, int prefix) {
+// 7x7 count tree: offset of row idx (2^(5-idx) words) in the tree's front part (idx >= 3) or rear part (idx < 3)
+__host__ __device__ constexpr uint32_t nz7_row(int idx) { return idx >= 3 ? 8u - (16u >> (idx - 2)) : 64u - (64u >> idx); }
+__host__ __device__ constexpr uint32_t m_nz7(int ci, int bin, int idx, int prefix) {
+    return (idx >= 3 ? M_NZ7T + (uint32_t)(ci * 10 + bin) * 8u : M_NZ7 + (uint32_t)(ci * 10 + bin) * 56u) + nz7_row(idx) + (uint32_t)prefix;
+}
+__host__ __device__ constexpr uint32_t m_nze(int vertical, int ci, int eob, int nzb, int idx, int prefix) {
     return M_NZE + (((((vertical * 2 + ci) * 8 + eob) * 8 + nzb) * 3 + idx) << 2) + prefix;
 }
 // (a position-innermost variant of the three big tables was measured slower for both kernel A and the decode kernel, and dropped)
-__host__ __device__ inline uint32_t m_resn(int ci, int coord, int bin) { return M_RESN + (((ci * 64 + coord) * 10 + bin) << 4); }
-__host__ __device__ inline uint32_t m_exp7(int ci, int bin, int zz, int bsr) { return M_EXP7 + ((((ci * 10 + bin) * 49 + zz) * 12 + bsr) << 4); }
-__host__ __device__ inline uint32_t m_expx(int ci, int ne, int zig15, int bsr) { return M_EXPX + ((((ci * 8 + ne) * 15 + zig15) * 12 + bsr) << 4); }
-__host__ __device__ inline uint32_t m_resdc(int lenmxm) { return M_RESDC + (lenmxm << 4); }
-__host__ __device__ inline uint32_t m_expdc(int a, int b) { return M_EXPDC + ((a * 17 + b) << 4); }
-__host__ __device__ inline uint32_t m_sign(int ci, int a, int b) { return M_SIGN + (ci * 4 + a) * 12 + b; }
-__host__ __device__ inline uint32_t m_thr(int ci, int ctx, int len) { return M_THR + (((ci * 256 + ctx) * 8 + len) << 7); }
+__host__ __device__ constexpr uint32_t m_resn(int ci, int coord, int bin) { return M_RESN + (((ci * 64 + coord) * 10 + bin) << 4); }
+// exponent tables: the address of word k = 0 of a context (its head)
+__host__ __device__ constexpr uint32_t m_exp7(int ci, int bin, int zz, int bsr) { return M_EXP7 + ((((ci * 10 + bin) * 49 + zz) * 12 + bsr) << 2); }
+__host__ __device__ constexpr uint32_t m_expx(int ci, int ne, int zig15, int bsr) { return M_EXPX + ((((ci * 8 + ne) * 15 + zig15) * 12 + bsr) << 2); }
+__host__ __device__ constexpr uint32_t m_expdc(int a, int b) { return M_EXPDC + ((a * 17 + b) << 2); }
+// word k (0..10) of the exponent chain whose head is at `head`
+__host__ __device__ constexpr uint32_t m_exp_word(uint32_t head, int k) { return k < 4 ? head + (uint32_t)k : M_EXPT + 2u * (head - M_EXPH) + (uint32_t)(k - 4); }
+// word k + 1 of the chain, from the address of word k (k < 10)
+__host__ __device__ constexpr uint32_t m_exp_next(uint32_t addr, int k) { return k == 3 ? M_EXPT + 2u * (addr - M_EXPH) - 6u : addr + 1u; }
+__host__ __device__ constexpr uint32_t m_resdc(int lenmxm) { return M_RESDC + lenmxm * 10; }
+__host__ __device__ constexpr uint32_t m_sign(int ci, int a, int b) { return M_SIGN + (ci * 4 + a) * 12 + b; }
+__host__ __device__ constexpr uint32_t m_thr(int ci, int ctx, int len) { return M_THR + (((ci * 256 + ctx) * 8 + len) << 7); }
+
+// no two tables overlap: the last word each index function can produce lies below the start of the next table
+static_assert(m_sign(1, 3, 11) < M_RESDC && m_resdc(11) + 9 < M_NZ7T && m_nz7(1, 9, 5, 0) < M_EXPH, "front region tables overlap");
+static_assert(m_exp_word(m_expdc(11, 16), 3) < M_EXP7 && m_exp_word(m_exp7(1, 9, 48, 11), 3) < M_EXPX &&
+              m_exp_word(m_expx(1, 7, 14, 11), 3) < M_EXPT, "exponent heads overlap");
+static_assert(m_exp_word(m_expdc(0, 0), 4) == M_EXPT && m_exp_next(m_exp_word(m_exp7(1, 2, 3, 4), 3), 3) == m_exp_word(m_exp7(1, 2, 3, 4), 4) &&
+              m_exp_word(m_expx(1, 7, 14, 11), 10) < M_NZ7, "exponent tails overlap");
+static_assert(m_nz7(1, 9, 0, 31) < M_NZE && m_nze(1, 1, 7, 7, 2, 3) < M_RESN && m_resn(1, 63, 9) + 15 < M_THR &&
+              m_thr(1, 255, 7) + 127 < M_TOTAL, "model tables overlap");
 
 // ------------------------------------------------------------------------------------------------------
 // Small constant tables (reference: src/vp8/util/aligned_block.hh:32-55, src/vp8/model/jpeg_meta.hh:72-170 row 9).

@@ -79,7 +79,7 @@ __device__ __forceinline__ uint32_t dec_get(Decoder& d, uint32_t addr) {
 // exponent unary + sign + residual bits of one coefficient (decoder.cc:212-240); returns the signed value
 __device__ __forceinline__ int dec_coef_plain(Decoder& d, uint32_t exp_addr, uint32_t sign_addr, uint32_t res_addr, int& len_out) {
     int len = 0;
-    while (len < 11) { if (!dec_get(d, exp_addr + len)) break; ++len; }
+    while (len < 11) { if (!dec_get(d, m_exp_word(exp_addr, len))) break; ++len; }
     len_out = len;
     if (len == 0) return 0;
     bool neg = !dec_get(d, sign_addr);
@@ -239,7 +239,7 @@ lep_decode_kernel(const ImageDesc* __restrict__ images, SegDesc* __restrict__ se
                             const int bsr = bitlen((uint32_t)min(iabs(prior), 1023));
                             const uint32_t ea = m_expx(ci, ne, zig15, bsr);
                             int len = 0;
-                            while (len < 11) { if (!dec_get(d, ea + len)) break; ++len; }
+                            while (len < 11) { if (!dec_get(d, m_exp_word(ea, len))) break; ++len; }
                             int v = 0;
                             if (len) {
                                 const int p16 = (int)(int16_t)prior;

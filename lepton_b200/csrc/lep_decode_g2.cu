@@ -10,7 +10,11 @@
 //   * end-of-block positions (eob_x / eob_y) are found by the lanes after the 7x7 loop instead of per decision, the
 //     residual / threshold table addresses are formed only when a coefficient turns out to need them;
 //   * the count trees are read as whole rows before their first bit, so no bit of a count waits for a load;
-//   * the stream window is topped up from a word fetched one refill ahead.
+//   * the stream window is topped up from a word fetched one refill ahead;
+//   * the front region of the model (M_HOT words: signs, DC residuals, DC exponent heads, top rows of the 7x7 count
+//     trees) lives in shared memory, one copy per group, zero-filled when the group takes a
+//     segment.  A branch address below M_HOT selects the group's shared copy, any other the model in global memory,
+//     through a generic pointer, so the step loops keep one load per candidate and no branch.
 //
 // Same job descriptors, model layout, work queue and results as lep_decode_group.cu.
 #include "lep_common.cuh"
@@ -106,16 +110,21 @@ __device__ __forceinline__ uint32_t g2_half8(uint4 v, uint32_t i) {
 __device__ __forceinline__ uint32_t g2_half4(uint2 v, uint32_t i) {
     return (((i & 2u) ? v.y : v.x) >> ((i & 1u) << 4)) & 0xffffu;
 }
-// the 7x7 count tree (m_nz7): rows 5..2 hold 1, 2, 4, 8 words at the row start and do not depend on a bit of the count,
-// so they are requested together, as early as the tree's base is known
+// the 7x7 count tree (m_nz7): rows 5..2 hold 1, 2, 4, 8 words and do not depend on a bit of the count, so they are
+// requested together, as early as the tree is known: rows 5..3 from the front region in shared memory (`top` = row 3),
+// row 2 from the tree's rear part in global memory (`rear` = row 0)
 struct G2NzTop { uint32_t r5, r4; uint2 r3; uint4 r2; };
-__device__ __forceinline__ G2NzTop g2_nz_top(const uint16_t* t) {
+__device__ __forceinline__ G2NzTop g2_nz_top(const uint16_t* top, const uint16_t* rear) {
     G2NzTop v;
-    v.r5 = t[5 << 5];
-    v.r4 = *reinterpret_cast<const uint32_t*>(t + (4 << 5));
-    v.r3 = *reinterpret_cast<const uint2*>(t + (3 << 5));
-    v.r2 = *reinterpret_cast<const uint4*>(t + (2 << 5));
+    v.r5 = top[nz7_row(5) - nz7_row(3)];
+    v.r4 = *reinterpret_cast<const uint32_t*>(top + (nz7_row(4) - nz7_row(3)));
+    v.r3 = *reinterpret_cast<const uint2*>(top);
+    v.r2 = *reinterpret_cast<const uint4*>(rear + nz7_row(2));
     return v;
+}
+// the branch word at `addr`: the group's shared copy of the front region, or the segment's model in global memory
+__device__ __forceinline__ uint16_t* g2_word(uint16_t* hot, uint16_t* model, uint32_t addr) {
+    return (addr < M_HOT ? hot : model) + addr;
 }
 // an edge count tree (m_nze): rows 2, 1, 0 of 1, 2, 4 words, 24 bytes in all
 struct G2EdgeTree { uint32_t r2, r1; uint2 r0; };
@@ -143,6 +152,11 @@ template <int G> struct G2Cfg {
     static constexpr int S = 32 / G;                                               // groups (thread-segments) per warp
     static constexpr int WARPS = (G >= 4) ? 4 : G;                                 // static shared memory stays under 48 KB
     static constexpr int THREADS = WARPS * 32;
+    static constexpr size_t HOT_BYTES = (size_t)WARPS * S * M_HOT * 2;          // dynamic shared memory: the groups' front regions
+    // static (s_rcp, s_a2r, s_nzbin, s_eb, s_grp) + dynamic shared memory: two CTAs stay resident on an SM (228 KB, 1 KB
+    // reserved per CTA), so that the 8192 segments of a 132-SM launch are all in flight at once
+    static constexpr size_t SMEM_BYTES = 512 * 4 + 64 + 64 + 2 * 52 * 4 + sizeof(G2GroupSmem) * WARPS * S + HOT_BYTES;
+    static_assert(SMEM_BYTES <= 113 * 1024, "two CTAs of the group kernel per SM");
 };
 
 template <int G> __device__ __forceinline__ int g2_sum(int v) {
@@ -188,6 +202,11 @@ lep_decode_g2_kernel(const ImageDesc* __restrict__ images, SegDesc* __restrict__
     __shared__ uint8_t s_nzbin[64];       // remaining non-zero count -> bin (jpeg_meta.hh:72-170 row 9)
     __shared__ uint32_t s_eb[2][52];      // [ci][remaining count]: base of the 7x7 exponent table slice of that bin
     __shared__ G2GroupSmem s_grp[G2Cfg<G>::WARPS * S];
+#ifndef LEPB200_EMU
+    extern __shared__ uint4 s_hot[];      // [group][M_HOT / 8]
+#else
+    static uint4 s_hot[G2Cfg<G>::HOT_BYTES / 16];
+#endif
     for (int i = threadIdx.x; i < 512; i += blockDim.x) s_rcp[i] = i < 2 ? 0u : (uint32_t)((0x100000000ull + i - 1) / i);
     for (int i = threadIdx.x; i < 64; i += blockDim.x) { s_a2r[i] = c_aligned_to_raster[i]; s_nzbin[i] = i < 50 ? c_nonzero_to_bin[i] : 0; }
     for (int i = threadIdx.x; i < 2 * 52; i += blockDim.x) {
@@ -200,7 +219,9 @@ lep_decode_g2_kernel(const ImageDesc* __restrict__ images, SegDesc* __restrict__
     const int gbase = lane & ~(G - 1);                    // first lane of the group
     const int slot = (blockIdx.x * G2Cfg<G>::WARPS + (threadIdx.x >> 5)) * S + lane / G;       // row buffer of this group
     G2GroupSmem& gs = s_grp[(threadIdx.x >> 5) * S + lane / G];
-    uint16_t* const eoff = reinterpret_cast<uint16_t*>(gs.tmp);          // 7x7: (zz * 12 + bsr) << 4
+    uint4* const hot4 = s_hot + (size_t)((threadIdx.x >> 5) * S + lane / G) * (M_HOT / 8);
+    uint16_t* const hot = reinterpret_cast<uint16_t*>(hot4);            // model words [0, M_HOT) of this group's segment
+    uint16_t* const eoff = reinterpret_cast<uint16_t*>(gs.tmp);          // 7x7: (zz * 12 + bsr) << 2
     uint32_t* const einfo = reinterpret_cast<uint32_t*>(gs.tmp) + 32;    // edges: g2_edge_info
     uint8_t* rowbuf = row_pool + (size_t)slot * row_pool_stride;
 
@@ -229,9 +250,9 @@ lep_decode_g2_kernel(const ImageDesc* __restrict__ images, SegDesc* __restrict__
     const int32_t* icx = nullptr;
     const int32_t* icy = nullptr;
     const uint8_t* mthr = nullptr;
-    // ---- the 7x7 count tree of the block to come: base and top rows, requested at the end of the previous block of the
-    //      row when it has one (in flight during phases (1) and (1b)), else in (1b)
-    uint32_t cnt_addr = 0;
+    // ---- the 7x7 count tree of the block to come: rows 3 and 0 (front and rear part) and the top rows, requested at the
+    //      end of the previous block of the row when it has one (in flight during phases (1) and (1b)), else in (1b)
+    uint32_t cnt_top = 0, cnt_rear = 0;
     G2NzTop nzt = {};
     bool cnt_ready = false;
 
@@ -259,6 +280,7 @@ lep_decode_g2_kernel(const ImageDesc* __restrict__ images, SegDesc* __restrict__
                         nzs0 = (bw0 + 15) & ~15; nzs1 = (bw1 + 15) & ~15;
                         need_row = true;
                         alive = true;
+                        for (int i = sub; i < (int)(M_HOT / 8); i += G) hot4[i] = make_uint4(0u, 0u, 0u, 0u);     // identity prior
                     }
                 }
             }
@@ -322,7 +344,7 @@ lep_decode_g2_kernel(const ImageDesc* __restrict__ images, SegDesc* __restrict__
             for (int k = 0; k < CPL / 2; ++k) reinterpret_cast<uint32_t*>(rcur)[sub * (CPL / 2) + k] = 0u;
         }
         __syncwarp();
-        // ---- (1b) exponent offsets of the 49 inner positions: compute_aavrg (model.hh:895-924) -> bit length -> (zz*12+bsr)<<4
+        // ---- (1b) exponent offsets of the 49 inner positions: compute_aavrg (model.hh:895-924) -> bit length -> (zz*12+bsr)<<2
         if (alive) {
             for (int zz = sub; zz < 49; zz += G) {
                 const int coord = s_a2r[zz];
@@ -334,7 +356,7 @@ lep_decode_g2_kernel(const ImageDesc* __restrict__ images, SegDesc* __restrict__
                     const int16_t nb = has_left ? rleft[coord] : rabove[coord];
                     pr = (uint32_t)iabs((int)(int16_t)((uint32_t)iabs(nb) & 0xffff));
                 }
-                eoff[zz] = (uint16_t)((zz * 12 + bitlen(min(pr, 1023u))) << 4);
+                eoff[zz] = (uint16_t)((zz * 12 + bitlen(min(pr, 1023u))) << 2);
             }
             if (!cnt_ready) {
                 const int nz_above = has_above ? (int)rnz[x] : 0;
@@ -342,15 +364,15 @@ lep_decode_g2_kernel(const ImageDesc* __restrict__ images, SegDesc* __restrict__
                 if (has_above && !has_left) ctx = (nz_above + 1) / 2;
                 else if (has_left && !has_above) ctx = (nz_left + 1) / 2;
                 else if (has_left && has_above) ctx = (nz_above + nz_left + 2) / 4;
-                cnt_addr = m_nz7(ci, s_nzbin[ctx], 0, 0);
-                nzt = g2_nz_top(model + cnt_addr);
+                cnt_top = m_nz7(ci, s_nzbin[ctx], 3, 0); cnt_rear = m_nz7(ci, s_nzbin[ctx], 0, 0);
+                nzt = g2_nz_top(hot + cnt_top, model + cnt_rear);
             }
         }
         cnt_ready = false;
         __syncwarp();
 
         // ---- (2a) the 7x7 non-zero count: six decisions, every live group in step (decoder.cc:175-184).  Level idx of the
-        //      tree is the row cnt_addr + idx * 32, indexed by the bits above it.  Rows 5..2 are in registers already; the
+        //      tree is the row m_nz7(ci, bin, idx, 0), indexed by the bits above it.  Rows 5..2 are in registers already; the
         //      8 words of row 1 that the first bit leaves possible, and of row 0 after the second bit, are requested three
         //      decisions before they are used.  No word of the tree is read twice, so nothing needs forwarding.
         {
@@ -364,11 +386,12 @@ lep_decode_g2_kernel(const ImageDesc* __restrict__ images, SegDesc* __restrict__
                 uint32_t split = 0, bit = 0;
                 if (alive) bit = g2_bit(br, s_rcp, mw, split);
                 const uint32_t p1 = (prefix << 1) | bit;
-                if (alive && idx == 5) r1 = *reinterpret_cast<const uint4*>(model + cnt_addr + (1u << 5) + (p1 << 3));
-                if (alive && idx == 4) r0 = *reinterpret_cast<const uint4*>(model + cnt_addr + (p1 << 3));
+                if (alive && idx == 5) r1 = *reinterpret_cast<const uint4*>(model + cnt_rear + nz7_row(1) + (p1 << 3));
+                if (alive && idx == 4) r0 = *reinterpret_cast<const uint4*>(model + cnt_rear + nz7_row(0) + (p1 << 3));
                 if (idx >= 4) G2_EMU_BARRIER();
                 if (alive) {
-                    model[cnt_addr + ((uint32_t)idx << 5) + prefix] = (uint16_t)g2_model_word(mw, bit);
+                    uint16_t* const row = idx >= 3 ? hot + cnt_top + (nz7_row(idx) - nz7_row(3)) : model + cnt_rear + nz7_row(idx);
+                    row[prefix] = (uint16_t)g2_model_word(mw, bit);
                     g2_update(br, split, bit);
                     prefix = p1;
                 }
@@ -397,7 +420,7 @@ lep_decode_g2_kernel(const ImageDesc* __restrict__ images, SegDesc* __restrict__
                 addr = eb + eoff[0];
                 a1 = addr + 1; a0 = eb + eoff[1];          // after the first exponent bit of position 0
             }
-            uint32_t mw = busy ? model[addr] : 0u;
+            uint32_t mw = busy ? *g2_word(hot, model, addr) : 0u;
             while (__any_sync(FULL, busy)) {
                 if (busy) {
                     // ---- on the chain
@@ -405,10 +428,10 @@ lep_decode_g2_kernel(const ImageDesc* __restrict__ images, SegDesc* __restrict__
                     const uint32_t bit = g2_bit(br, s_rcp, mw, split);
                     const uint32_t naddr = bit ? a1 : a0;
                     const bool nbusy = bit ? b1 : b0;
-                    uint32_t mwn = nbusy ? model[naddr] : 0u;
+                    uint32_t mwn = nbusy ? *g2_word(hot, model, naddr) : 0u;
                     // ---- in the shadow of that load: write-back, window, grammar state, decoded value
                     const uint32_t neww = g2_model_word(mw, bit);
-                    model[addr] = (uint16_t)neww;                  // all lanes of the group store the same value
+                    *g2_word(hot, model, addr) = (uint16_t)neww;   // all lanes of the group store the same value
                     if (naddr == addr) mwn = neww;
                     g2_update(br, split, bit);
                     ++nd;
@@ -440,7 +463,7 @@ lep_decode_g2_kernel(const ImageDesc* __restrict__ images, SegDesc* __restrict__
                         const uint32_t cont_a = inS ? m_resn(ci, s_a2r[zz], s_nzbin[left_nz]) + (uint32_t)(len - 2) : addr - 1;
                         const uint32_t common = fin ? nextN : cont_a;
                         const bool commonB = fin ? !doneN : true;
-                        a1 = inE ? (len < 10 ? addr + 1 : sign_addr) : common;
+                        a1 = inE ? (len < 10 ? m_exp_next(addr, len) : sign_addr) : common;
                         a0 = inE ? (len == 0 ? s_eb[ci][left_nz] + eoff[zn] : sign_addr) : common;
                         b1 = inE ? true : commonB;
                         b0 = inE ? (len == 0 ? !lastpos : true) : commonB;
@@ -510,18 +533,19 @@ lep_decode_g2_kernel(const ImageDesc* __restrict__ images, SegDesc* __restrict__
             int ln = 0, st = G2_EXP, len = 0, ri = 0, val = 0;
             bool neg = false;
             uint32_t addr = 0, e = 0, so = 1, thr_base = 0, a0 = 0, a1 = 0;
-            const uint32_t expx_base = M_EXPX + (uint32_t)((ci * 8) * 15 * 12 * 16) + (uint32_t)(vert * 7 * 12 * 16);
-            const uint32_t sign_base = M_SIGN + (uint32_t)(ci * 48);
+            const uint32_t expx_base = m_expx(ci, 0, vert * 7, 0);
+            const uint32_t sign_base = m_sign(ci, 0, 0);
             const int cstep = vert ? 8 : 1;                       // raster distance between the coefficients of this edge
-            constexpr uint32_t NE_STRIDE = 15 * 12 * 16;          // exponent contexts of one remaining-count value
+            constexpr uint32_t NE_STRIDE = 15 * 12 * 4;           // exponent heads of one remaining-count value
+            constexpr uint32_t POS_STRIDE = 12 * 4;               // exponent heads of one position
             bool busy = alive && ne > 0, b0 = busy, b1 = busy;
             if (busy) {
                 e = einfo[vert * 7];
-                addr = expx_base + (uint32_t)ne * NE_STRIDE + ((e & 15u) << 4);
+                addr = expx_base + (uint32_t)ne * NE_STRIDE + ((e & 15u) << 2);
                 a1 = addr + 1;
-                a0 = expx_base + (uint32_t)ne * NE_STRIDE + (uint32_t)(12 * 16) + ((einfo[vert * 7 + 1] & 15u) << 4);
+                a0 = expx_base + (uint32_t)ne * NE_STRIDE + POS_STRIDE + ((einfo[vert * 7 + 1] & 15u) << 2);
             }
-            uint32_t mw = busy ? model[addr] : 0u;
+            uint32_t mw = busy ? *g2_word(hot, model, addr) : 0u;
             while (__any_sync(FULL, busy)) {
                 if (busy) {
                     // ---- on the chain (see the 7x7 loop)
@@ -529,10 +553,10 @@ lep_decode_g2_kernel(const ImageDesc* __restrict__ images, SegDesc* __restrict__
                     const uint32_t bit = g2_bit(br, s_rcp, mw, split);
                     const uint32_t naddr = bit ? a1 : a0;
                     const bool nbusy = bit ? b1 : b0;
-                    uint32_t mwn = nbusy ? model[naddr] : 0u;
+                    uint32_t mwn = nbusy ? *g2_word(hot, model, naddr) : 0u;
                     // ---- in the shadow of that load
                     const uint32_t neww = g2_model_word(mw, bit);
-                    model[addr] = (uint16_t)neww;
+                    *g2_word(hot, model, addr) = (uint16_t)neww;
                     if (naddr == addr) mwn = neww;                 // saturated threshold index: the same branch twice in a row
                     g2_update(br, split, bit);
                     ++nd;
@@ -565,7 +589,7 @@ lep_decode_g2_kernel(const ImageDesc* __restrict__ images, SegDesc* __restrict__
                         const int mt2 = (int)((e >> 6) & 7u);
                         const bool lastpos = ln == 6;
                         const bool doneN = ne == 1 || lastpos;                   // after the non-zero coefficient in progress
-                        const uint32_t nxt = (uint32_t)((ln + 1) * (12 * 16)) + ((einfo[vert * 7 + min(ln + 1, 6)] & 15u) << 4);
+                        const uint32_t nxt = (uint32_t)(ln + 1) * POS_STRIDE + ((einfo[vert * 7 + min(ln + 1, 6)] & 15u) << 2);
                         const uint32_t nextN = expx_base + (uint32_t)(ne - 1) * NE_STRIDE + nxt;
                         const uint32_t rb = m_resn(ci, (ln + 1) * cstep, ne);
                         const bool inE = st == G2_EXP, inS = st == G2_SIGN, inT = st == G2_THR;
@@ -579,7 +603,7 @@ lep_decode_g2_kernel(const ImageDesc* __restrict__ images, SegDesc* __restrict__
                         const uint32_t c1 = fin ? nextN : thr ? tb + so1 : rest;
                         const bool cb = fin ? !doneN : true;
                         const uint32_t sa = sign_base + ((e >> 4) & 3u) * 12u + (e & 15u);
-                        a1 = inE ? (len < 10 ? addr + 1 : sa) : c1;
+                        a1 = inE ? (len < 10 ? m_exp_next(addr, len) : sa) : c1;
                         a0 = inE ? (len == 0 ? expx_base + (uint32_t)ne * NE_STRIDE + nxt : sa) : c0;
                         b1 = inE ? true : cb;
                         b0 = inE ? (len == 0 ? !lastpos : true) : cb;
@@ -668,16 +692,16 @@ lep_decode_g2_kernel(const ImageDesc* __restrict__ images, SegDesc* __restrict__
             bool neg = false;
             uint32_t addr = dc_exp, a0 = dc_exp, a1 = dc_exp + 1;
             bool busy = alive, b0 = false, b1 = busy;
-            uint32_t mw = busy ? model[addr] : 0u;
+            uint32_t mw = busy ? *g2_word(hot, model, addr) : 0u;
             while (__any_sync(FULL, busy)) {
                 if (busy) {
                     uint32_t split;
                     const uint32_t bit = g2_bit(br, s_rcp, mw, split);
                     const uint32_t naddr = bit ? a1 : a0;
                     const bool nbusy = bit ? b1 : b0;
-                    uint32_t mwn = nbusy ? model[naddr] : 0u;
+                    uint32_t mwn = nbusy ? *g2_word(hot, model, naddr) : 0u;
                     const uint32_t neww = g2_model_word(mw, bit);
-                    model[addr] = (uint16_t)neww;
+                    *g2_word(hot, model, addr) = (uint16_t)neww;
                     if (naddr == addr) mwn = neww;
                     g2_update(br, split, bit);
                     ++nd;
@@ -699,7 +723,7 @@ lep_decode_g2_kernel(const ImageDesc* __restrict__ images, SegDesc* __restrict__
                         const bool inE = st == G2_EXP, inS = st == G2_SIGN;
                         const bool fin = inS ? len < 2 : ri == 0;
                         const uint32_t common = inS ? dc_res + (uint32_t)(len - 2) : addr - 1;
-                        a1 = inE ? (len < 10 ? addr + 1 : dc_sign) : common;
+                        a1 = inE ? (len < 10 ? m_exp_next(addr, len) : dc_sign) : common;
                         a0 = inE ? dc_sign : common;
                         b1 = inE ? true : !fin;
                         b0 = inE ? len != 0 : !fin;
@@ -752,8 +776,9 @@ lep_decode_g2_kernel(const ImageDesc* __restrict__ images, SegDesc* __restrict__
                 need_row = true;
             } else {                      // the 7x7 count tree of the next block is known now (phase (1b) with a left neighbour)
                 const int nza = has_above ? (int)rnz[x + 1] : 0;
-                cnt_addr = m_nz7(ci, s_nzbin[has_above ? (nza + nz + 2) / 4 : (nz + 1) / 2], 0, 0);
-                nzt = g2_nz_top(model + cnt_addr);
+                const int bin = s_nzbin[has_above ? (nza + nz + 2) / 4 : (nz + 1) / 2];
+                cnt_top = m_nz7(ci, bin, 3, 0); cnt_rear = m_nz7(ci, bin, 0, 0);
+                nzt = g2_nz_top(hot + cnt_top, model + cnt_rear);
                 cnt_ready = true;
                 ++x; pc ^= 1; pa ^= 1;
             }

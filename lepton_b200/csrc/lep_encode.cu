@@ -2,7 +2,7 @@
 //
 // Work decomposition (new; the reference runs one CPU thread per segment, src/lepton/vp8_encoder.cc:239-445):
 //   * persistent grid, one WARP per Lepton thread-segment, segments pulled from a global work queue
-//     (largest first), the warp's 1.58 MB probability model zero-filled by the warp itself;
+//     (largest first), the warp's 1.45 MB probability model zero-filled by the warp itself;
 //   * kernel A (lep_encode_kernel) codes TWO blocks (x, x + 1) per iteration in two phases
 //       1. lane-parallel SYMBOLISATION.  Nothing in the encoder's context computation depends on coder state
 //          (SURVEY.md section 7, hard part 1), so the warp computes, for both blocks, the neighbour priors /
@@ -65,7 +65,7 @@ __device__ __forceinline__ uint32_t expand_item(const uint4 d, int pos) {      /
     if (d.x >> 31) return d.y;
     const int len = (int)((d.x >> 20) & 15u), nexp = min(len + 1, 11);
     const int k = pos - (int)(d.z >> 20);
-    if (k < nexp) return ((d.x & 0xfffffu) + (uint32_t)k) | ((uint32_t)(len != k) << 31);
+    if (k < nexp) return m_exp_word(d.x & 0xfffffu, k) | ((uint32_t)(len != k) << 31);
     if (k == nexp) return (d.y & 0xfffffu) | (((d.x >> 24) & 1u) << 31);
     const int ib = len - 2 - (k - nexp - 1);                  // residual bit index, MSB first
     const uint32_t av = d.y >> 20;
