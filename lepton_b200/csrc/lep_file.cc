@@ -203,6 +203,19 @@ struct ChunkState {
     std::vector<lepb200_result> files;           // ... and the finished files (pinned memory of the chunk's context)
 };
 
+// The device Huffman decoder's job for one JPEG (sc.rows stays the caller's): geometry, and with a set-up the entropy bytes,
+// restart interval and tables; without one a placeholder that only gets its plane slot.
+void fill_jpeg_scan(const Jpeg& j, const GpuScanSetup* gs, lepb200_jpeg_scan& sc) {
+    lepb200_huffrow* rows = sc.rows;
+    memset(&sc, 0, sizeof(sc));
+    sc.rows = rows;
+    sc.ncmp = j.ncmp; sc.mcuh = j.mcuh; sc.mcuv = j.mcuv;
+    for (int t = 0; t < j.ncmp && t < 3; ++t) { sc.H[t] = j.cmp[t].H; sc.V[t] = j.cmp[t].V; sc.nch[t] = j.cmp[t].nch; sc.ncv[t] = j.cmp[t].ncv; }
+    if (!gs) return;
+    sc.entropy = j.huff.data(); sc.nbytes = (uint32_t)j.huff.size(); sc.rsti = gs->rsti;
+    for (int t = 0; t < j.ncmp; ++t) { sc.dc[t] = gs->dc[t]; sc.ac[t] = gs->ac[t]; }
+}
+
 }  // namespace
 
 int lepb200_compress_jpegs(lepb200_codec* c, const lepb200_buffer* jpegs, int n, lepb200_result* out) {
@@ -350,16 +363,8 @@ int lepb200_compress_jpegs(lepb200_codec* c, const lepb200_buffer* jpegs, int n,
             const int i = s.idx[q];
             const Jpeg& j = *s.js[i];
             lepb200_jpeg_scan& sc = s.scans[q];
-            memset(&sc, 0, sizeof(sc));
-            sc.ncmp = j.ncmp; sc.mcuh = j.mcuh; sc.mcuv = j.mcuv;
-            for (int t = 0; t < j.ncmp && t < 3; ++t) { sc.H[t] = j.cmp[t].H; sc.V[t] = j.cmp[t].V; sc.nch[t] = j.cmp[t].nch; sc.ncv[t] = j.cmp[t].ncv; }
+            fill_jpeg_scan(j, eligible[i] ? &setups[i] : nullptr, sc);
             if (!eligible[i]) continue;              // placeholder: plane slot only
-            const GpuScanSetup& gs = setups[i];
-            sc.entropy = j.huff.data(); sc.nbytes = (uint32_t)j.huff.size(); sc.rsti = gs.rsti;
-            for (int t = 0; t < j.ncmp; ++t) {
-                memcpy(sc.dc[t].bits, gs.dc_bits[t], 17); memcpy(sc.dc[t].vals, gs.dc_vals[t], 256);
-                memcpy(sc.ac[t].bits, gs.ac_bits[t], 17); memcpy(sc.ac[t].vals, gs.ac_vals[t], 256);
-            }
             s.rowbuf[q].resize((size_t)j.mcuv + 1);
             sc.rows = s.rowbuf[q].data();
             s.any_gpu_huffman = true;
@@ -559,8 +564,7 @@ static void fill_henc_image(const LepFile& lf, GpuRecodeSetup& gs, lepb200_henc_
     he.rsti = gs.rsti; he.padbit = (uint8_t)j.padbit;
     for (int t = 0; t < j.ncmp; ++t) {
         he.H[t] = j.cmp[t].H; he.V[t] = j.cmp[t].V;
-        memcpy(he.dc[t].bits, gs.dc_bits[t], 17); memcpy(he.dc[t].vals, gs.dc_vals[t], 256);
-        memcpy(he.ac[t].bits, gs.ac_bits[t], 17); memcpy(he.ac[t].vals, gs.ac_vals[t], 256);
+        he.dc[t] = gs.dc[t]; he.ac[t] = gs.ac[t];
     }
     const int luma_mul = j.cmp[0].bcv / j.mcuv;
     he.nseg = lf.nseg;
@@ -1069,16 +1073,7 @@ int lepb200_host_jpeg_scan(lepb200_jpeg* h, lepb200_jpeg_scan* sc) {
     const Jpeg& j = h->j;
     GpuScanSetup gs;
     if (!gpu_scan_setup(j, gs)) return LEPB200_ERR_INVALID;
-    lepb200_huffrow* rows = sc->rows;
-    memset(sc, 0, sizeof(*sc));
-    sc->rows = rows;
-    sc->ncmp = j.ncmp; sc->mcuh = j.mcuh; sc->mcuv = j.mcuv; sc->rsti = gs.rsti;
-    for (int t = 0; t < j.ncmp && t < 3; ++t) {
-        sc->H[t] = j.cmp[t].H; sc->V[t] = j.cmp[t].V; sc->nch[t] = j.cmp[t].nch; sc->ncv[t] = j.cmp[t].ncv;
-        memcpy(sc->dc[t].bits, gs.dc_bits[t], 17); memcpy(sc->dc[t].vals, gs.dc_vals[t], 256);
-        memcpy(sc->ac[t].bits, gs.ac_bits[t], 17); memcpy(sc->ac[t].vals, gs.ac_vals[t], 256);
-    }
-    sc->entropy = j.huff.data(); sc->nbytes = (uint32_t)j.huff.size();
+    fill_jpeg_scan(j, &gs, *sc);
     return LEPB200_OK;
 }
 

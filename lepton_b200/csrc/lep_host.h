@@ -44,7 +44,7 @@ struct Handoff {
 };
 
 struct Component {
-    int jid = 0, H = 0, V = 0, tq = 0, td = 0, ta = 0;   // H = horizontal sampling (reference "sfv"), V = vertical ("sfh")
+    int jid = 0, H = 0, V = 0, tq = 0;                   // H = horizontal sampling (reference "sfv"), V = vertical ("sfh")
     int bch = 0, bcv = 0, bc = 0, nch = 0, ncv = 0, mbs = 0;
 };
 
@@ -129,9 +129,10 @@ bool decode_scans(Jpeg& j, int16_t* const planes[4]);
 // ---- GPU Huffman path helpers
 struct GpuScanSetup {
     int rsti = 0;
-    uint8_t dc_bits[3][17], dc_vals[3][256], ac_bits[3][17], ac_vals[3][256];
+    lepb200_hufftable dc[3], ac[3];  // tables selected by the SOS for each component (frame order == scan order)
 };
-bool gpu_scan_setup(const Jpeg& j, GpuScanSetup& out);
+// sos_end (optional) receives the end of the SOS segment inside j.hdr.
+bool gpu_scan_setup(const Jpeg& j, GpuScanSetup& out, size_t* sos_end = nullptr);
 Handoff handoff_from_state(const Jpeg& j, uint32_t bitpos, int mcu_y, const int16_t lastdc[3]);
 
 // ---- container ----------------------------------------------------------------------------------
@@ -178,9 +179,7 @@ bool read_lep(const uint8_t* data, size_t n, LepFile& lf, bool lazy = false);
 bool brotli_available();          // libbrotlidec could be loaded: container versions 2 / 4 (brotli header blob) are read
 // Set-up for re-encoding the scan on the GPU (lepb200_huffman_encode_resident): false when the file needs the host
 // re-encoder (progressive, truncated, several scans, scan order != frame order, restart-marker budget).
-struct GpuRecodeSetup {
-    int rsti = 0;
-    uint8_t dc_bits[3][17], dc_vals[3][256], ac_bits[3][17], ac_vals[3][256];
+struct GpuRecodeSetup : GpuScanSetup {
     size_t hpos = 0;                 // end of the first SOS segment inside hdr
     uint32_t scan_bytes = 0;         // entropy-coded bytes of the scan in the original file
 };

@@ -3,6 +3,7 @@ planes and thread-segment splits, and the container writer must reproduce the re
 reference's own segment streams (so header blob, zlib stream, handoffs, mux packets and trailer are all pinned)."""
 import hashlib
 import os
+import zlib
 
 import numpy as np
 import pytest
@@ -105,6 +106,53 @@ def test_device_reencode_layout_and_assembly(name):
     sos = jpg.rfind(b"\xff\xda", 0, off)
     assert sos >= 0 and off == sos + 2 + int.from_bytes(jpg[sos + 2:sos + 4], "big")     # right behind the SOS segment
     assert hl.assemble(jpg[off:off + n]) == jpg
+
+
+def _with_header(lep, edit):
+    """`lep` with the JPEG header of its header blob replaced by edit(header).  The recorded JPEG size follows the header,
+    so that only the header's contents can make a re-encoder refuse the file."""
+    zlen = int.from_bytes(lep[24:28], "little")
+    blob = zlib.decompress(lep[28:28 + zlen])
+    assert blob[:3] == b"HDR"
+    hs = int.from_bytes(blob[3:7], "little")
+    hdr = edit(blob[7:7 + hs])
+    z = zlib.compress(b"HDR" + len(hdr).to_bytes(4, "little") + hdr + blob[7 + hs:])
+    size = int.from_bytes(lep[20:24], "little") + len(hdr) - hs
+    return lep[:20] + size.to_bytes(4, "little") + len(z).to_bytes(4, "little") + z + lep[28 + zlen:]
+
+
+def _at_first_sos(hdr, seg, replace):
+    pos = 0
+    while hdr[pos + 1] != 0xDA:
+        pos += 2 + int.from_bytes(hdr[pos + 2:pos + 4], "big")
+    end = pos + 2 + int.from_bytes(hdr[pos + 2:pos + 4], "big")
+    return hdr[:pos] + seg + hdr[end if replace else pos:]
+
+
+SHORT_DHT = b"\xff\xc4\x00\x03\x00"       # a table's class / id byte, then none of its 16 count bytes
+BAD_CLASS_DHT = b"\xff\xc4\x00\x03\x24"   # table class 2, id 4
+
+
+@pytest.mark.parametrize("name,edit", [
+    # the baseline re-encoder reads the header up to the first SOS: here it finds none and reads on to the header's end
+    ("android", lambda h: _at_first_sos(h, SHORT_DHT, replace=True)),
+    # the multi-scan re-encoder reads every segment, this one last
+    ("androidprogressive", lambda h: h + SHORT_DHT),
+    ("android", lambda h: _at_first_sos(h, BAD_CLASS_DHT, replace=False)),
+    ("androidprogressive", lambda h: h + BAD_CLASS_DHT),
+], ids=["short_dht_baseline", "short_dht_progressive", "dht_class_baseline", "dht_class_progressive"])
+def test_reencoders_refuse_malformed_dht_in_lep_header(name, edit):
+    """The header of a .lep is untrusted input.  A DHT segment that ends inside a table's count bytes, or that names a table
+    class or id out of range, is refused by the reference's header parser ("size mismatch in dht marker", parse_jfif_jpg,
+    jpgcoder.cc:4558-4590), and so by both host re-encoders: the container reads, but neither re-encode nor the device
+    re-encode layout takes the file, and no byte outside the header is read."""
+    from lepton_b200 import HostJpeg, HostLep, LeptonB200Error
+    planes = HostJpeg(open(os.path.join(GOLDEN, name + ".jpg"), "rb").read()).coef_image().planes
+    hl = HostLep(_with_header(open(os.path.join(GOLDEN, name + ".lep"), "rb").read(), edit))
+    assert hl.status == 0, hl.error
+    assert hl.scan_layout() == (0, 0)
+    with pytest.raises(LeptonB200Error, match="dht"):
+        hl.recode(planes)
 
 
 @pytest.mark.timeout(60)
