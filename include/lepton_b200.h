@@ -277,6 +277,16 @@ void lepb200_codec_set_even_split(lepb200_codec* codec, int on);
  * (environment LEPB200_ZLIB0_HOST_ADLER=1: by the host, over every byte).  Statuses do not change; lepb200_compress_jpegs
  * ignores the setting, as the reference does.  0 (default): plain JPEG bytes. */
 void lepb200_codec_set_zlib0(lepb200_codec* codec, int on);
+/* -embedding=N (jpgcoder.cc:1135-1137, read_jpeg :2275-2282): offset >= 0 makes lepb200_compress_jpegs take every input as a
+ * JPEG whose SOI sits at byte `offset` of a larger file.  The bytes in front of it go to the container's PGE section and
+ * are written back in front of the SOI on restore, bytes after the EOI to its GRB section as always; the coded JPEG takes
+ * the same device path as a plain one.  As in the reference, the two bytes at `offset` are not looked at, an offset past
+ * the end of the input is ASSERTION_FAILURE (1), and 0 gives the plain .lep.  Negative (default): inputs start at their SOI. */
+void lepb200_codec_set_embedding(lepb200_codec* codec, long long offset);
+/* -d (rebuild_header_jpg, jpgcoder.cc:3797-3800, 4848-4888): 1 = the container keeps only the header segments the
+ * coefficients are coded with (DQT, DHT, DRI, SOF0-2, SOS); APPn, COM and the rest are dropped, so the restored JPEG is
+ * shorter than the input (with verification on, such a file fails with 41 as in the reference).  0 (default): all kept. */
+void lepb200_codec_set_discard_meta(lepb200_codec* codec, int on);
 /* device milliseconds of the last chunk's GPU Huffman-decode kernel (diagnostic) */
 double lepb200_codec_last_huffman_ms(const lepb200_codec* codec);
 /* files of the last lepb200_decompress_leps call whose scan was Huffman-encoded on the device (the rest went through the host re-encoder) */
@@ -304,6 +314,10 @@ typedef struct lepb200_jpeg lepb200_jpeg;
 int lepb200_host_jpeg_open(const uint8_t* data, size_t len, lepb200_jpeg** out, int32_t* status);
 int lepb200_host_jpeg_open_threads(const uint8_t* data, size_t len, int min_threads, int max_threads, lepb200_jpeg** out, int32_t* status);
 int lepb200_host_jpeg_open_split(const uint8_t* data, size_t len, int min_threads, int max_threads, int even_split, lepb200_jpeg** out, int32_t* status);
+/* ... with -embedding=N (embedding >= 0; negative: none) and -d (discard_meta = 1), as lepb200_codec_set_embedding /
+ * lepb200_codec_set_discard_meta */
+int lepb200_host_jpeg_open_embedded(const uint8_t* data, size_t len, int min_threads, int max_threads, int even_split,
+                                    long long embedding, int discard_meta, lepb200_jpeg** out, int32_t* status);
 const char* lepb200_host_jpeg_error(const lepb200_jpeg* h);
 int lepb200_host_jpeg_image(lepb200_jpeg* h, lepb200_image* img);
 /* the scan as lepb200_huffman_decode_to_device takes it (de-stuffed entropy bytes, tables, geometry; pointers valid until

@@ -64,6 +64,7 @@ _EXPORTS = [
     "lepb200_decompress_leps", "lepb200_host_lep_open", "lepb200_host_lep_error", "lepb200_host_lep_image",
     "lepb200_host_lep_stream", "lepb200_host_lep_recode", "lepb200_host_lep_close", "lepb200_host_frontend_seconds",
     "lepb200_codec_set_zlib0", "lepb200_huffman_encode_adler32", "lepb200_host_lep_zlib0", "lepb200_host_zlib0_frame",
+    "lepb200_codec_set_embedding", "lepb200_codec_set_discard_meta", "lepb200_host_jpeg_open_embedded",
 ]
 
 
@@ -350,6 +351,13 @@ def _bind_file_api(L):
     L.lepb200_host_jpeg_open_threads.restype = ctypes.c_int
     L.lepb200_host_jpeg_open_split.argtypes = [ctypes.c_char_p, ctypes.c_size_t, ctypes.c_int, ctypes.c_int, ctypes.c_int, ctypes.POINTER(vp), ctypes.POINTER(ctypes.c_int32)]
     L.lepb200_host_jpeg_open_split.restype = ctypes.c_int
+    L.lepb200_host_jpeg_open_embedded.argtypes = [ctypes.c_char_p, ctypes.c_size_t, ctypes.c_int, ctypes.c_int, ctypes.c_int,
+                                                  ctypes.c_longlong, ctypes.c_int, ctypes.POINTER(vp), ctypes.POINTER(ctypes.c_int32)]
+    L.lepb200_host_jpeg_open_embedded.restype = ctypes.c_int
+    L.lepb200_codec_set_embedding.argtypes = [vp, ctypes.c_longlong]
+    L.lepb200_codec_set_embedding.restype = None
+    L.lepb200_codec_set_discard_meta.argtypes = [vp, ctypes.c_int]
+    L.lepb200_codec_set_discard_meta.restype = None
     L.lepb200_codec_set_even_split.argtypes = [vp, ctypes.c_int]
     L.lepb200_codec_set_even_split.restype = None
     L.lepb200_codec_set_verify.argtypes = [vp, ctypes.c_int]
@@ -388,13 +396,18 @@ def _bind_file_api(L):
 class HostJpeg:
     """Host stages only (no GPU): parse + Huffman-decode a JPEG, expose it as a CoefImage, assemble a .lep."""
 
-    def __init__(self, data: bytes, min_threads: int = 1, max_threads: int = 8, even_split: bool = False):
+    def __init__(self, data: bytes, min_threads: int = 1, max_threads: int = 8, even_split: bool = False,
+                 embedding: Optional[int] = None, discard_meta: bool = False):
+        """embedding=N (-embedding=N): the JPEG's SOI sits at byte N of `data`; discard_meta=True (-d): the container keeps only
+        the header segments the coefficients are coded with."""
         self._L = lib()
         _bind_file_api(self._L)
         self._h = ctypes.c_void_p()
         st = ctypes.c_int32()
         self._data = data
-        self._L.lepb200_host_jpeg_open_split(data, len(data), min_threads, max_threads, 1 if even_split else 0, ctypes.byref(self._h), ctypes.byref(st))
+        self._L.lepb200_host_jpeg_open_embedded(data, len(data), min_threads, max_threads, 1 if even_split else 0,
+                                                -1 if embedding is None else embedding, 1 if discard_meta else 0,
+                                                ctypes.byref(self._h), ctypes.byref(st))
         self.status = st.value
         self.error = self._L.lepb200_host_jpeg_error(self._h).decode()
 
@@ -535,11 +548,14 @@ def zlib0_frame(data: bytes) -> bytes:
 
 class LeptonB200FileCodec:
     """JPEG bytes -> .lep bytes for a batch of files; host threads + one GPU.  zlib0=True (-zlib0): decompress hands every
-    JPEG out as a zlib stream of stored blocks, as containers with the zeta magic (CE B6) always are."""
+    JPEG out as a zlib stream of stored blocks, as containers with the zeta magic (CE B6) always are.  embedding=N
+    (-embedding=N): compress takes every input as a JPEG whose SOI sits at byte N, keeping the bytes in front of it in the
+    container.  discard_meta=True (-d): the container keeps only the header segments the coefficients are coded with."""
 
     def __init__(self, device: int = 0, host_threads: int = 0, chunk_images: int = 0, gpu_huffman: bool = True,
                  allow_progressive: bool = True, min_encode_threads: int = 1, max_encode_threads: int = 8,
-                 even_split: bool = False, verify: bool = False, zlib0: bool = False):
+                 even_split: bool = False, verify: bool = False, zlib0: bool = False, embedding: Optional[int] = None,
+                 discard_meta: bool = False):
         self._L = lib()
         _bind_file_api(self._L)
         self._c = ctypes.c_void_p()
@@ -554,6 +570,8 @@ class LeptonB200FileCodec:
         self._L.lepb200_codec_set_even_split(self._c, 1 if even_split else 0)                      # -evensplit
         self._L.lepb200_codec_set_verify(self._c, 1 if verify else 0)                              # -verify (reference default) / -skipverify
         self._L.lepb200_codec_set_zlib0(self._c, 1 if zlib0 else 0)                                # -zlib0
+        self._L.lepb200_codec_set_embedding(self._c, -1 if embedding is None else embedding)         # -embedding=N
+        self._L.lepb200_codec_set_discard_meta(self._c, 1 if discard_meta else 0)                  # -d
 
     def close(self):
         if self._c:

@@ -42,6 +42,8 @@ struct lepb200_codec {
     bool verify = false;           // -verify: decode every .lep again and compare with the input before handing it out
     bool allow_progressive = true; // false: -rejectprogressive (files that are not single-scan-interleaved baseline exit with code 8)
     bool zlib0 = false;            // -zlib0: restored JPEGs are handed out as zlib streams of stored blocks
+    long long embedding = -1;      // -embedding=N (>= 0): every input is a JPEG whose SOI sits at byte N; the bytes in front are kept
+    bool discard_meta = false;     // -d: the container keeps only the header segments the coefficients are coded with
     void* arena[4] = {nullptr, nullptr, nullptr, nullptr};  // pinned host memory for coefficient planes, one per in-flight chunk
     size_t arena_cap[4] = {0, 0, 0, 0};
     std::vector<std::vector<uint8_t>> outputs;
@@ -156,6 +158,8 @@ void lepb200_codec_set_allow_progressive(lepb200_codec* c, int on) { if (c) c->a
 void lepb200_codec_set_even_split(lepb200_codec* c, int on) { if (c) c->even_split = on != 0; }
 void lepb200_codec_set_verify(lepb200_codec* c, int on) { if (c) c->verify = on != 0; }
 void lepb200_codec_set_zlib0(lepb200_codec* c, int on) { if (c) c->zlib0 = on != 0; }
+void lepb200_codec_set_embedding(lepb200_codec* c, long long offset) { if (c) c->embedding = offset < 0 ? -1 : offset; }
+void lepb200_codec_set_discard_meta(lepb200_codec* c, int on) { if (c) c->discard_meta = on != 0; }
 void lepb200_codec_set_encode_threads(lepb200_codec* c, int min_threads, int max_threads) {
     if (!c) return;
     c->min_encode_threads = (unsigned)std::min(std::max(min_threads, 1), 8);
@@ -229,7 +233,7 @@ int lepb200_compress_jpegs(lepb200_codec* c, const lepb200_buffer* jpegs, int n,
     c->t_front = c->t_gpu = c->t_back = 0;
     // ---- chunk boundaries
     std::vector<size_t> need(n);
-    parallel_for(n, c->nthreads, [&](int i) { need[i] = peek_plane_bytes(jpegs[i].data, jpegs[i].len); });
+    parallel_for(n, c->nthreads, [&](int i) { need[i] = peek_plane_bytes(jpegs[i].data, jpegs[i].len, c->embedding); });
     // Chunks: up to `concurrent` of them run at the same time, each on its own context (stream + device arenas), so
     // that the latency-bound kernels of one chunk (Huffman decode, range coder) and its host stages lie under the
     // issue-bound kernel A of another.  A large call is cut into that many chunks of about equal plane bytes; the
@@ -312,7 +316,7 @@ int lepb200_compress_jpegs(lepb200_codec* c, const lepb200_buffer* jpegs, int n,
                 const lepb200_buffer& in = jpegs[s.begin + i];
                 if (stage) { j.huff.attach(stage + soff[i], soff[i + 1] - soff[i] - 16); memset(stage + soff[i], 0, 16); }
                 if (need[s.begin + i] > c->plane_cap / (size_t)W) { j.status = NOT_HANDLED; j.error = "image larger than the per-chunk device memory budget"; continue; }
-                const bool parsed = parse_jpeg(in.data, in.len, j);
+                const bool parsed = parse_jpeg(in.data, in.len, j, c->embedding, c->discard_meta);
                 if (stage) memset(stage + soff[i] + j.huff.size(), 0, 16);          // the decoder reads whole words past the end
                 if (parsed && stage && gpu_scan_setup(j, setups[i])) eligible[i] = 1;
             }
@@ -893,7 +897,7 @@ int lepb200_host_lep_scan_layout(lepb200_lep* h, uint32_t* scan_offset, uint32_t
     if (!h || h->lf.status || !scan_offset || !scan_bytes) return LEPB200_ERR_INVALID;
     GpuRecodeSetup gs;
     if (!gpu_recode_setup(h->lf, gs)) { *scan_offset = 0; *scan_bytes = 0; return LEPB200_OK; }
-    *scan_offset = (uint32_t)(2 + gs.hpos);
+    *scan_offset = (uint32_t)(h->lf.j.prefix.size() + 2 + gs.hpos);
     *scan_bytes = gs.scan_bytes;
     return LEPB200_OK;
 }
@@ -1045,10 +1049,15 @@ int lepb200_host_jpeg_open_threads(const uint8_t* data, size_t len, int min_thre
 }
 
 int lepb200_host_jpeg_open_split(const uint8_t* data, size_t len, int min_threads, int max_threads, int even_split, lepb200_jpeg** out, int32_t* status) {
+    return lepb200_host_jpeg_open_embedded(data, len, min_threads, max_threads, even_split, -1, 0, out, status);
+}
+
+int lepb200_host_jpeg_open_embedded(const uint8_t* data, size_t len, int min_threads, int max_threads, int even_split,
+                                    long long embedding, int discard_meta, lepb200_jpeg** out, int32_t* status) {
     if (!out || !data) return LEPB200_ERR_INVALID;
     lepb200_jpeg* h = new lepb200_jpeg();
     *out = h;
-    if (parse_jpeg(data, len, h->j)) {
+    if (parse_jpeg(data, len, h->j, embedding < 0 ? -1 : embedding, discard_meta != 0)) {
         h->store.resize(h->j.ncmp);
         for (int c = 0; c < h->j.ncmp; ++c) {
             h->store[c].assign((size_t)h->j.cmp[c].bc * 64, 0);

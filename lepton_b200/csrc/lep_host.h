@@ -93,11 +93,12 @@ struct Jpeg {
     std::vector<uint8_t> hdr;        // every marker segment after SOI, in file order ("hdrdata")
     HuffBuf huff;                    // entropy-coded bytes of all scans, de-stuffed, RST markers removed ("huffdata")
     std::vector<uint8_t> grb;        // bytes from EOI on ("grbgdata"); empty when exactly FF D9
+    std::vector<uint8_t> prefix;     // -embedding=N: the N bytes in front of the JPEG's SOI ("prefix_grbgdata", 'PGE' section)
     std::vector<std::pair<uint32_t, uint32_t>> offs;   // (position in huff, position in file) ("huff_input_offsets")
     std::vector<uint32_t> rst_cnt;   // restart markers seen per scan
     std::vector<uint8_t> rst_err;    // trailing bogus restart markers per scan
     bool early_eof = false;
-    uint32_t filesize = 0;
+    uint32_t filesize = 0;           // the whole input, prefix included ("jpgfilesize")
     // ---- frame (setup_imginfo_jpg, jpgcoder.cc:4450-4540)
     int jpegtype = 0;                // 1 sequential, 2 progressive
     int width = 0, height = 0, ncmp = 0;
@@ -115,12 +116,16 @@ struct Jpeg {
     std::string error;
 };
 
-// Parse the container level of a JPEG file (everything except Huffman decoding).  `data` starts at SOI.
-bool parse_jpeg(const uint8_t* data, size_t n, Jpeg& j);
+// Parse the container level of a JPEG file (everything except Huffman decoding).  `data` starts at SOI unless
+// `embedding` >= 0 (-embedding=N, read_jpeg jpgcoder.cc:2275-2282): then the JPEG's two SOI bytes sit at byte `embedding`,
+// the bytes in front of them become j.prefix, and, as in the reference, the two bytes there are skipped without a look.
+// File positions (handoffs, filesize) count from the start of `data`, prefix included.  `discard_meta` (-d,
+// rebuild_header_jpg :4848-4888) keeps only the header segments the coefficients need (DQT, DHT, DRI, SOF0-2, SOS).
+bool parse_jpeg(const uint8_t* data, size_t n, Jpeg& j, long long embedding = -1, bool discard_meta = false);
 // Frame geometry + quantisation tables from j.hdr (setup_imginfo_jpg); used by both directions.
 bool parse_frame(Jpeg& j);
-// Header-only peek: total (256-byte padded) bytes of all coefficient planes, 0 if unknown.
-size_t peek_plane_bytes(const uint8_t* data, size_t n);
+// Header-only peek: total (256-byte padded) bytes of all coefficient planes, 0 if unknown.  `embedding` as for parse_jpeg.
+size_t peek_plane_bytes(const uint8_t* data, size_t n, long long embedding = -1);
 // Bytes of coefficient plane c (AlignedBlock order).
 inline size_t plane_bytes(const Jpeg& j, int c) { return (size_t)j.cmp[c].bc * 128; }
 // Huffman-decode all scans into planes (pre-zeroed, AlignedBlock order) and record the per-row handoffs.

@@ -62,9 +62,17 @@ bool HuffTable::build() {
 // ------------------------------------------------------------------------------------------------
 bool parse_frame(Jpeg& j);
 
-bool parse_jpeg(const uint8_t* data, size_t n, Jpeg& j) {
-    if (n < 4 || data[0] != 0xFF || data[1] != 0xD8) return fail(j, UNSUPPORTED_JPEG, "not a JPEG (no SOI)");
+bool parse_jpeg(const uint8_t* data, size_t n, Jpeg& j, long long embedding, bool discard_meta) {
     size_t pos = 2;                       // jpg_ident_offset (jpgcoder.cc:1809)
+    if (embedding < 0) {
+        if (n < 4 || data[0] != 0xFF || data[1] != 0xD8) return fail(j, UNSUPPORTED_JPEG, "not a JPEG (no SOI)");
+    } else {
+        // the reference reads the two bytes that tell the file type, then N more, and keeps the first N of them as the
+        // prefix: the JPEG's own SOI is taken on trust (jpgcoder.cc:2275-2281)
+        if (n < 2 || (unsigned long long)n - 2 < (unsigned long long)embedding) return fail(j, ASSERTION_FAILURE, "embedding offset beyond the end of the file");
+        j.prefix.assign(data, data + embedding);
+        pos = (size_t)embedding + 2;
+    }
     uint8_t type = 0, seg0 = 0, seg1 = 0;
     bool eof_called = false;
     int scnc = 0;
@@ -140,7 +148,11 @@ bool parse_jpeg(const uint8_t* data, size_t n, Jpeg& j) {
         if (j.grb.size() == 2 && j.grb[0] == 0xFF && j.grb[1] == 0xD9) j.grb.clear();
     }
     j.filesize = (uint32_t)n;
-    return parse_frame(j);
+    if (!parse_frame(j)) return false;
+    // -d: the reference drops the other segments when it writes the container (write_ujpg, jpgcoder.cc:3797-3800); the
+    // decode never reads them, so they can go here
+    if (discard_meta) j.hdr = coding_segments(j.hdr);
+    return true;
 }
 
 // setup_imginfo_jpg + the SOF/DQT cases of parse_jfif_jpg
@@ -224,9 +236,14 @@ bool parse_frame(Jpeg& j) {
 
 // Quick marker walk up to the first SOF: total bytes of the coefficient planes (0 if not determinable here;
 // the full parse then reports the precise error).  Used to lay out the pinned plane arena before decoding.
-size_t peek_plane_bytes(const uint8_t* data, size_t n) {
-    if (n < 4 || data[0] != 0xFF || data[1] != 0xD8) return 0;
+size_t peek_plane_bytes(const uint8_t* data, size_t n, long long embedding) {
     size_t pos = 2;
+    if (embedding < 0) {
+        if (n < 4 || data[0] != 0xFF || data[1] != 0xD8) return 0;
+    } else {
+        if ((unsigned long long)n < (unsigned long long)embedding + 2) return 0;
+        pos = (size_t)embedding + 2;
+    }
     while (pos + 4 <= n) {
         if (data[pos] != 0xFF) return 0;
         const uint8_t type = data[pos + 1];

@@ -199,8 +199,15 @@ bool read_lep(const uint8_t* d, size_t n, LepFile& lf, bool lazy) {
                 j.trunc_bc[c] = (int)tbc;
             }
             p += 31;
-        } else if (!memcmp(m, "PGR", 3) || !memcmp(m, "PGE", 3) || !memcmp(m, "SIZ", 3)) {
-            return lfail(lf, NOT_HANDLED, "prefix garbage / embedded JPEG sections are not handled");
+        } else if (!memcmp(m, "PGE", 3)) {
+            // -embedding=N: the bytes in front of the embedded JPEG, written back in front of its SOI (read_ujpg :4292-4308)
+            if (!need(7)) return lfail(lf, SHORT_READ, "short PGE");
+            uint32_t k = rd32(m + 3);
+            if (!need(7 + (size_t)k)) return lfail(lf, SHORT_READ, "short PGE");
+            j.prefix.assign(m + 7, m + 7 + k);
+            p += 7 + (size_t)k;
+        } else if (!memcmp(m, "PGR", 3) || !memcmp(m, "SIZ", 3)) {
+            return lfail(lf, NOT_HANDLED, "-startbyte slice sections (PGR / SIZ) are not handled");
         } else {
             return lfail(lf, UNSUPPORTED_JPEG, "unknown data found in header blob");
         }
@@ -356,6 +363,17 @@ inline void encode_block_seq(FastWriter& bw, const int16_t* blk, const HuffTable
 
 bool recode_scans(const LepFile& lf, const int16_t* const planes[4], std::vector<uint8_t>& out, std::string& err);
 
+namespace {
+// A re-created JPEG of `n` bytes (counted with its prefix) against the size the container promises: the same, or shorter
+// when the header holds nothing but the coding segments, as -d leaves it -- the container keeps the size of the file
+// with its metadata, and the reference restores the file without it.
+bool size_checks(const LepFile& lf, size_t n, std::string& err) {
+    if (n == lf.jpeg_size || (n < lf.jpeg_size && coding_segments(lf.j.hdr).size() == lf.j.hdr.size())) return true;
+    err = "re-created JPEG has the wrong size";
+    return false;
+}
+}  // namespace
+
 bool gpu_recode_setup(const LepFile& lf, GpuRecodeSetup& out) {
     const Jpeg& j = lf.j;
     if (lf.flag != 'Z' || lf.has_eee || !gpu_scan_setup(j, out, &out.hpos)) return false;
@@ -365,7 +383,7 @@ bool gpu_recode_setup(const LepFile& lf, GpuRecodeSetup& out) {
     const unsigned nrst = out.rsti ? (unsigned)(j.mcuc - 1) / (unsigned)out.rsti : 0u;
     if (lf.rst_cnt_set && !j.rst_cnt.empty() && j.rst_cnt[0] < nrst) return false;
     const size_t trailing = j.rst_err.empty() ? 0 : 2 * (size_t)j.rst_err[0];
-    const size_t fixed = 2 + j.hdr.size() + j.grb.size() + trailing;
+    const size_t fixed = j.prefix.size() + 2 + j.hdr.size() + j.grb.size() + trailing;
     if ((size_t)lf.jpeg_size <= fixed) return false;
     out.scan_bytes = (uint32_t)(lf.jpeg_size - fixed);
     return true;
@@ -424,9 +442,10 @@ bool assemble_baseline(const LepFile& lf, const GpuRecodeSetup& gs, const uint8_
         const unsigned cum = gs.rsti ? (unsigned)(j.mcuh * j.mcuv - 1) / gs.rsti : 0;
         for (unsigned i = 0; i < j.rst_err[0] && nrst + 2 <= sizeof(rst); ++i) { rst[nrst++] = 0xFF; rst[nrst++] = (uint8_t)(0xD0 + ((cum + i) & 7)); }
     }
-    // the JPEG in pieces: [0, 2) in front of the scan, [2] the scan, [3, 6) behind it
-    const std::pair<const uint8_t*, size_t> pieces[6] = {
-        {soi, 2}, {h.data(), gs.hpos}, {scan, gs.scan_bytes}, {rst, nrst}, {h.data() + gs.hpos, h.size() - gs.hpos}, {j.grb.data(), j.grb.size()}};
+    // the JPEG in pieces: [0, 3) in front of the scan (prefix of an embedded JPEG, SOI, header), [3] the scan, [4, 7) behind it
+    const std::pair<const uint8_t*, size_t> pieces[7] = {
+        {j.prefix.data(), j.prefix.size()}, {soi, 2}, {h.data(), gs.hpos}, {scan, gs.scan_bytes}, {rst, nrst},
+        {h.data() + gs.hpos, h.size() - gs.hpos}, {j.grb.data(), j.grb.size()}};
     size_t total = 0;
     for (const auto& pc : pieces) total += pc.second;
     if (total != lf.jpeg_size) { err = "re-created JPEG has the wrong size"; out.clear(); return false; }
@@ -446,10 +465,10 @@ bool assemble_baseline(const LepFile& lf, const GpuRecodeSetup& gs, const uint8_
     // the device took the scan's sum; the host sums the few header and trailer bytes and combines the three
     uLong head = 1, tail = 1;
     size_t ntail = 0;
-    for (int k = 0; k < 6; ++k) {
+    for (int k = 0; k < 7; ++k) {
         w.put(pieces[k].first, pieces[k].second);
-        if (k < 2) head = adler32(head, pieces[k].first, (uInt)pieces[k].second);
-        if (k > 2) { tail = adler32(tail, pieces[k].first, (uInt)pieces[k].second); ntail += pieces[k].second; }
+        if (k < 3) head = adler32(head, pieces[k].first, (uInt)pieces[k].second);
+        if (k > 3) { tail = adler32(tail, pieces[k].first, (uInt)pieces[k].second); ntail += pieces[k].second; }
     }
     uLong a = adler32_combine(head, scan_adler, (z_off_t)gs.scan_bytes);
     a = adler32_combine(a, tail, (z_off_t)ntail);
@@ -478,6 +497,7 @@ bool recode_baseline(const LepFile& lf, const int16_t* const planes[4], std::vec
     const int rsti = t.rsti;
     out.clear();
     out.reserve((size_t)lf.jpeg_size + 64);
+    out.insert(out.end(), j.prefix.begin(), j.prefix.end());       // embedded JPEG: the prefix, then SOI and header (recoder.cc:449-456)
     out.push_back(0xFF); out.push_back(0xD8);
     out.insert(out.end(), h.begin(), h.begin() + hpos);
 
@@ -535,8 +555,7 @@ bool recode_baseline(const LepFile& lf, const int16_t* const planes[4], std::vec
     // cut exactly where the file ended (str_out->set_bound, recoder.cc:699-700, 880-886)
     if (lf.jpeg_size >= j.grb.size() && out.size() > lf.jpeg_size - j.grb.size()) out.resize(lf.jpeg_size - j.grb.size());
     out.insert(out.end(), j.grb.begin(), j.grb.end());
-    if (out.size() != lf.jpeg_size) { err = "re-created JPEG has the wrong size"; return false; }
-    return true;
+    return size_checks(lf, out.size(), err);
 }
 
 
@@ -592,6 +611,8 @@ bool recode_scans(const LepFile& lf, const int16_t* const planes[4], std::vector
     size_t hpos = 0;
     out.clear();
     out.reserve((size_t)lf.jpeg_size + 64);
+    // no prefix: the reference's multi-scan restore (recode_jpeg / merge_jpeg_streaming, jpgcoder.cc:2562-2740, 3309) writes
+    // SOI and header only, so an embedded progressive JPEG comes back without the bytes in front of it
     out.push_back(0xFF); out.push_back(0xD8);
     FastWriter bw(out, (size_t)lf.jpeg_size);
     ProgWriter pw(bw);
@@ -748,8 +769,7 @@ bool recode_scans(const LepFile& lf, const int16_t* const planes[4], std::vector
     if (pw.bad) { err = "coefficients not expressible with the scan's huffman tables"; return false; }
     if (lf.jpeg_size >= j.grb.size() && out.size() > lf.jpeg_size - j.grb.size()) out.resize(lf.jpeg_size - j.grb.size());
     out.insert(out.end(), j.grb.begin(), j.grb.end());
-    if (out.size() != lf.jpeg_size) { err = "re-created JPEG has the wrong size"; return false; }
-    return true;
+    return size_checks(lf, out.size() + j.prefix.size(), err);
 }
 
 }  // namespace lephost

@@ -95,15 +95,24 @@ struct ScanTables {
 
 enum class Seg { sos, end, error };
 
+// The marker segment at `pos` of a header blob (FF, type, two length bytes, payload): its type and its length with the
+// marker counted.  False when fewer than four bytes are left.  The length may run past the end of an untrusted blob.
+inline bool segment_at(const std::vector<uint8_t>& h, size_t pos, uint8_t& type, size_t& len) {
+    if (pos + 4 > h.size()) return false;
+    type = h[pos + 1];
+    len = 2 + be16(&h[pos + 2]);
+    return true;
+}
+
 // parse_jfif_jpg (jpgcoder.cc:4545-4680) for DHT, DRI and SOS: reads j.hdr from `pos` up to and including the next SOS.
 // Returns Seg::sos with `pos` behind the SOS and `sc` filled, Seg::end with `pos` at the < 4 bytes left when there is no
 // further SOS, or Seg::error with `err` set.  Nothing outside a segment is read: a DRI shorter than its two bytes reads
 // zero for the missing ones, like the reference; everything else short is refused.
 inline Seg read_to_sos(const Jpeg& j, size_t& pos, ScanTables& t, ScanInfo& sc, const char*& err) {
     const std::vector<uint8_t>& h = j.hdr;
-    while (pos + 4 <= h.size()) {
-        const uint8_t type = h[pos + 1];
-        const size_t len = 2 + be16(&h[pos + 2]);
+    uint8_t type;
+    size_t len;
+    while (segment_at(h, pos, type, len)) {
         if (pos + len > h.size()) { err = "truncated header segment"; return Seg::error; }      // the header of a .lep is untrusted input
         const uint8_t* seg = &h[pos];
         pos += len;
@@ -148,6 +157,19 @@ inline Seg read_to_sos(const Jpeg& j, size_t& pos, ScanTables& t, ScanInfo& sc, 
         }
     }
     return Seg::end;
+}
+
+// rebuild_header_jpg (jpgcoder.cc:4848-4888), -d: the segments the coefficients are coded with -- DQT, DHT, DRI, SOF0-2
+// and SOS -- in file order; everything else (APPn, COM, ...) is dropped.
+inline std::vector<uint8_t> coding_segments(const std::vector<uint8_t>& h) {
+    std::vector<uint8_t> out;
+    out.reserve(h.size());
+    uint8_t type;
+    size_t len;
+    for (size_t pos = 0; segment_at(h, pos, type, len) && pos + len <= h.size(); pos += len)
+        if (type == 0xDA || type == 0xC4 || type == 0xDB || type == 0xC0 || type == 0xC1 || type == 0xC2 || type == 0xDD)
+            out.insert(out.end(), h.begin() + pos, h.begin() + pos + len);
+    return out;
 }
 
 // Every table the scan codes with is defined (jpgcoder.cc:2858-2868).
