@@ -295,7 +295,11 @@ int lepb200_codec_last_gpu_recoded(const lepb200_codec* codec);
 void lepb200_codec_last_timing(const lepb200_codec* codec, double* front_s, double* gpu_s, double* back_s);
 /* n JPEG files in, n .lep files out */
 int lepb200_compress_jpegs(lepb200_codec* codec, const lepb200_buffer* jpegs, int n, lepb200_result* out);
-/* n .lep files in, n JPEG files out (byte-identical to the originals) */
+/* n .lep files in, n JPEG files out (byte-identical to the originals).  An input may be a stream of concatenated .lep files
+ * (`cat a.lep b.lep`, -lepcat files): out[i] is then the concatenation of its members' JPEGs -- for zlib0 output ONE zlib
+ * stream over all of them, as the reference writes -- and every member is one image of the call's batches.  The status of
+ * such an input is that of its first member that fails; then it gets no data (the reference has written the members in
+ * front of it by then). */
 int lepb200_decompress_leps(lepb200_codec* codec, const lepb200_buffer* leps, int n, lepb200_result* out);
 
 /* ---- several GPUs from one process: codecs[k] was created on its own device.  The files are dealt to the codecs
@@ -354,6 +358,19 @@ int lepb200_host_lep_assemble(lepb200_lep* h, const uint8_t* scan, size_t scan_l
 void lepb200_host_lep_close(lepb200_lep* h);
 /* 1 when the container opened with lepb200_host_lep_open carries the zeta magic CE B6 (its JPEG is restored as a zlib stream) */
 int lepb200_host_lep_zlib0(const lepb200_lep* h);
+/* Streams of concatenated .lep files (`cat a.lep b.lep`, the reference's -lepcat files; process_file, jpgcoder.cc:1867-1898):
+ * lepb200_decompress_leps restores every member of every input as one image of its batch.  lepb200_host_lep_members lists the
+ * members of `data` as that walk finds them: returns their number and writes up to `cap` entries.  The walk stops at the
+ * first member that fails (its status is non-zero); a stream ends behind a member without an EOF marker (container version
+ * 1), where fewer than 6 bytes follow the marker, or where the 2 bytes behind the member's 4-byte size trailer are not the
+ * first member's magic.  lepb200_host_lep_open_member opens member `index` like lepb200_host_lep_open opens a file. */
+typedef struct {
+    int32_t status;          /* 0, or the reference ExitCode the member fails with */
+    uint32_t jpeg_size;      /* size of the member's JPEG as its container records it */
+    int32_t nseg;            /* thread-segments */
+} lepb200_lep_member;
+int lepb200_host_lep_members(const uint8_t* data, size_t len, lepb200_lep_member* out, int cap);
+int lepb200_host_lep_open_member(const uint8_t* data, size_t len, int index, lepb200_lep** out, int32_t* status);
 /* test hook: the zlib stream lepb200_codec_set_zlib0 hands out for the `len` bytes at `data`.  Returns its length; writes it
  * to `out` only when cap is at least that length. */
 size_t lepb200_host_zlib0_frame(const uint8_t* data, size_t len, uint8_t* out, size_t cap);

@@ -65,6 +65,7 @@ _EXPORTS = [
     "lepb200_host_lep_stream", "lepb200_host_lep_recode", "lepb200_host_lep_close", "lepb200_host_frontend_seconds",
     "lepb200_codec_set_zlib0", "lepb200_huffman_encode_adler32", "lepb200_host_lep_zlib0", "lepb200_host_zlib0_frame",
     "lepb200_codec_set_embedding", "lepb200_codec_set_discard_meta", "lepb200_host_jpeg_open_embedded",
+    "lepb200_host_lep_members", "lepb200_host_lep_open_member",
 ]
 
 
@@ -390,6 +391,10 @@ def _bind_file_api(L):
     L.lepb200_host_lep_recode.restype = ctypes.c_int
     L.lepb200_host_lep_close.argtypes = [vp]
     L.lepb200_host_lep_close.restype = None
+    L.lepb200_host_lep_members.argtypes = [ctypes.c_char_p, ctypes.c_size_t, ctypes.c_void_p, ctypes.c_int]
+    L.lepb200_host_lep_members.restype = ctypes.c_int
+    L.lepb200_host_lep_open_member.argtypes = [ctypes.c_char_p, ctypes.c_size_t, ctypes.c_int, ctypes.POINTER(vp), ctypes.POINTER(ctypes.c_int32)]
+    L.lepb200_host_lep_open_member.restype = ctypes.c_int
     L._file_api_bound = True
 
 
@@ -459,13 +464,17 @@ class HostLep:
     """Decode-side host stages only (no GPU): parse a .lep, expose geometry / splits / segment streams, and
     re-create the JPEG bytes from coefficient planes."""
 
-    def __init__(self, data: bytes):
+    def __init__(self, data: bytes, member: Optional[int] = None):
+        """member=k opens the k-th member of a stream of concatenated .lep files (see lep_members)."""
         self._L = lib()
         _bind_file_api(self._L)
         self._h = ctypes.c_void_p()
         st = ctypes.c_int32()
         self._data = data
-        self._L.lepb200_host_lep_open(data, len(data), ctypes.byref(self._h), ctypes.byref(st))
+        if member is None:
+            self._L.lepb200_host_lep_open(data, len(data), ctypes.byref(self._h), ctypes.byref(st))
+        elif self._L.lepb200_host_lep_open_member(data, len(data), member, ctypes.byref(self._h), ctypes.byref(st)) != 0:
+            raise LeptonB200Error("the stream has no member %d" % member)
         self.status = st.value
         self.error = self._L.lepb200_host_lep_error(self._h).decode()
 
@@ -534,6 +543,23 @@ class HostLep:
         if self._L.lepb200_host_lep_recode(self._h, arr, ctypes.byref(d), ctypes.byref(n)) != 0:
             raise LeptonB200Error("recode failed: %s" % self._L.lepb200_host_lep_error(self._h).decode())
         return ctypes.string_at(d, n.value)
+
+
+class _LepMember(ctypes.Structure):
+    _fields_ = [("status", ctypes.c_int32), ("jpeg_size", ctypes.c_uint32), ("nseg", ctypes.c_int32)]
+
+
+def lep_members(data: bytes):
+    """The members of a stream of concatenated .lep files as decompress walks them (host code, no GPU): a list of
+    (status, JPEG size, thread-segments), up to and including the first member that fails."""
+    L = lib()
+    _bind_file_api(L)
+    n = L.lepb200_host_lep_members(data, len(data), None, 0)
+    if n < 0:
+        raise LeptonB200Error("lepb200_host_lep_members failed (%d)" % n)
+    arr = (_LepMember * max(n, 1))()
+    assert L.lepb200_host_lep_members(data, len(data), arr, n) == n
+    return [(m.status, m.jpeg_size, m.nseg) for m in arr[:n]]
 
 
 def zlib0_frame(data: bytes) -> bytes:

@@ -47,6 +47,7 @@ struct lepb200_codec {
     void* arena[4] = {nullptr, nullptr, nullptr, nullptr};  // pinned host memory for coefficient planes, one per in-flight chunk
     size_t arena_cap[4] = {0, 0, 0, 0};
     std::vector<std::vector<uint8_t>> outputs;
+    std::vector<std::vector<uint8_t>> joined;   // decompress: inputs of several members, their restored members concatenated
     std::string err;
     // timing of the last call (seconds): parse+huffman, gpu (upload+kernel+fetch), container
     double t_front = 0, t_gpu = 0, t_back = 0, t_huff_ms = 0;
@@ -599,17 +600,28 @@ int lepb200_decompress_leps(lepb200_codec* c, const lepb200_buffer* leps, int n,
     c->err.clear();
     c->t_front = c->t_gpu = c->t_back = 0;
     c->n_gpu_recoded = 0;
-    // ---- containers: fixed header, zlib'd JPEG header, handoffs, demux of the segment streams (all files, host threads)
+    // ---- containers: fixed header, zlib'd JPEG header, handoffs, demux of the segment streams (all files, host threads).
+    // Every input may be a stream of concatenated .lep files: each of its members is one image of the batch below, so the
+    // members of one input and those of different inputs share chunks, kernels and host stages alike.
     double t_parse = now_s();
-    std::vector<std::unique_ptr<LepFile>> all(n);
-    std::vector<size_t> pbytes(n, 0);
-    parallel_for(n, c->nthreads, [&](int i) {
-        all[i].reset(new LepFile());
-        if (read_lep(leps[i].data, leps[i].len, *all[i], /*lazy=*/true)) {    // mux packets stay where they are: gathered into the staging buffer
-            for (int q = 0; q < all[i]->j.ncmp; ++q) pbytes[i] += (plane_bytes(all[i]->j, q) + 255) & ~size_t(255);
-            if (pbytes[i] > c->plane_cap) { all[i]->status = NOT_HANDLED; all[i]->error = "image larger than the per-chunk device memory budget"; pbytes[i] = 0; }
-        }
+    std::vector<std::vector<std::unique_ptr<LepFile>>> members(n);
+    parallel_for(n, c->nthreads, [&](int i) { read_lep_members(leps[i].data, leps[i].len, members[i], /*lazy=*/true); });   // mux packets stay where they are: gathered into the staging buffer
+    std::vector<int> first(n + 1, 0);                 // members of input i: images first[i] .. first[i + 1] - 1
+    for (int i = 0; i < n; ++i) first[i + 1] = first[i] + (int)members[i].size();
+    const int nim = first[n];
+    std::vector<std::unique_ptr<LepFile>> all(nim);
+    std::vector<uint8_t> zjoin(nim, 0);               // 1: a member of an input of several members that goes out as one zlib stream
+    for (int i = 0; i < n; ++i) {
+        const bool z = members[i].size() > 1 && (c->zlib0 || members[i][0]->zlib0);
+        for (size_t m = 0; m < members[i].size(); ++m) { zjoin[first[i] + m] = z; all[first[i] + m] = std::move(members[i][m]); }
+    }
+    std::vector<size_t> pbytes(nim, 0);
+    parallel_for(nim, c->nthreads, [&](int u) {
+        if (all[u]->status) return;
+        for (int q = 0; q < all[u]->j.ncmp; ++q) pbytes[u] += (plane_bytes(all[u]->j, q) + 255) & ~size_t(255);
+        if (pbytes[u] > c->plane_cap) { all[u]->status = NOT_HANDLED; all[u]->error = "image larger than the per-chunk device memory budget"; pbytes[u] = 0; }
     });
+    std::vector<uint32_t> member_adler(nim, 1);       // zjoin images: Adler-32 of the restored member
     c->t_front += now_s() - t_parse;
     mark("containers", -1, t_parse);
     // chunks of up to `plane_cap` bytes of coefficient planes (device memory: three contexts in flight).  The planes stay on the device
@@ -625,26 +637,27 @@ int lepb200_decompress_leps(lepb200_codec* c, const lepb200_buffer* leps, int n,
         // The two chunks in flight share the budget when a call does not fit in one.
         const size_t budget = c->gpu_huffman ? c->plane_cap : (size_t(6) << 30);
         size_t total = 0;
-        for (int i = 0; i < n; ++i) total += pbytes[i];
+        for (int i = 0; i < nim; ++i) total += pbytes[i];
         const size_t cap = total > budget ? budget / 2 : budget;
         const int chunk_max = std::max(1, c->chunk_images);
         int b0 = 0;
         size_t acc = 0;
-        for (int i = 0; i < n; ++i) {
+        for (int i = 0; i < nim; ++i) {
             if (i > b0 && (i - b0 >= chunk_max || acc + pbytes[i] > cap)) { ranges.emplace_back(b0, i); b0 = i; acc = 0; }
             acc += pbytes[i];
         }
-        ranges.emplace_back(b0, n);
+        ranges.emplace_back(b0, nim);
         W = std::max(1, std::min(std::min(2, c->concurrent), (int)ranges.size()));
     }
     keep_arenas_for(c, 2, W);
     const int pth = std::max(1, c->nthreads / W);
     const int nchunks = (int)ranges.size();
     // the output buffers keep their capacity from call to call (a fresh 1.5 GB of vectors per 4096-file call is 370 K
-    // page faults inside the container stage); every file's buffer is rewritten or cleared below
-    c->outputs.resize(n);
+    // page faults inside the container stage); every image's buffer is rewritten or cleared below.  Indices from here on
+    // are images (members), not inputs.
+    c->outputs.resize(nim);
     for (auto& o : c->outputs) o.clear();
-    std::vector<int> status(n, 0);
+    std::vector<int> status(nim, 0);
     struct DChunk {
         int begin = 0, end = 0;
         std::vector<std::unique_ptr<LepFile>> lf;
@@ -734,7 +747,7 @@ int lepb200_decompress_leps(lepb200_codec* c, const lepb200_buffer* leps, int n,
     // unless LEPB200_ZLIB0_HOST_ADLER=1, which has the host sum every byte (the route of host-encoded files) for comparison
     const bool zlib0_host_adler = getenv("LEPB200_ZLIB0_HOST_ADLER") && atoi(getenv("LEPB200_ZLIB0_HOST_ADLER")) != 0;
     auto out_mode = [&](const LepFile& lf, bool device_scan) {
-        if (!c->zlib0 && !lf.zlib0) return JpegOut::plain;
+        if (!c->zlib0 && !lf.zlib0) return JpegOut::plain;       // a member's magic is its stream's first member's
         return device_scan && !zlib0_host_adler ? JpegOut::zlib0_scan_adler : JpegOut::zlib0_host_adler;
     };
     auto gpu = [&](int k) {               // H2D of the streams + decode kernel + Huffman encode of the resident planes, all queued
@@ -759,7 +772,7 @@ int lepb200_decompress_leps(lepb200_codec* c, const lepb200_buffer* leps, int n,
         std::string err;
         c->n_gpu_recoded++;
         const LepFile& lf = *s.lf[li];
-        if (!assemble_baseline(lf, s.gsetup[q], s.henc[q].data, c->outputs[i], err, out_mode(lf, true), scan_adler)) { status[i] = NOT_HANDLED; c->outputs[i].clear(); }
+        if (!assemble_baseline(lf, s.gsetup[q], s.henc[q].data, c->outputs[i], err, out_mode(lf, true), scan_adler, zjoin[i] ? &member_adler[i] : nullptr)) { status[i] = NOT_HANDLED; c->outputs[i].clear(); }
     };
     auto fetch_back = [&](int k) {
         double t0 = now_s();
@@ -823,7 +836,7 @@ int lepb200_decompress_leps(lepb200_codec* c, const lepb200_buffer* leps, int n,
                     if (s.seg_status[t]) { status[i] = s.seg_status[t]; return; }
                 std::string err;
                 const LepFile& lf = *s.lf[li];
-                if (!recode_baseline(lf, s.planes[li].data(), c->outputs[i], err, out_mode(lf, false))) { status[i] = NOT_HANDLED; c->outputs[i].clear(); }
+                if (!recode_baseline(lf, s.planes[li].data(), c->outputs[i], err, out_mode(lf, false), zjoin[i] ? &member_adler[i] : nullptr)) { status[i] = NOT_HANDLED; c->outputs[i].clear(); }
             });
         }
         s.lf.clear();
@@ -847,11 +860,25 @@ int lepb200_decompress_leps(lepb200_codec* c, const lepb200_buffer* leps, int n,
             rc = cs[k].gpu_rc; c->err = lepb200_last_error(c->ctx2[k % W]);
             for (int i = ranges[k].first; i < ranges[k].second; ++i) if (!status[i]) status[i] = 33;       // ExitCode::OS_ERROR
         }
-    for (int i = 0; i < n; ++i) {
-        out[i].status = status[i];
-        out[i].data = status[i] ? nullptr : c->outputs[i].data();
-        out[i].len = status[i] ? 0 : c->outputs[i].size();
-    }
+    // back to inputs: the status of the first member that failed, else the members' JPEGs one after the other (one zlib
+    // stream over all of them for zlib0 output).  A single member's buffer is handed out as it is.
+    c->joined.resize(n);
+    parallel_for(n, c->nthreads, [&](int i) {
+        int st = 0;
+        for (int u = first[i]; u < first[i + 1] && !st; ++u) st = status[u];
+        std::vector<uint8_t>* o = &c->outputs[first[i]];
+        if (!st && first[i + 1] - first[i] > 1) {
+            std::vector<std::pair<const uint8_t*, size_t>> parts;
+            for (int u = first[i]; u < first[i + 1]; ++u) parts.emplace_back(c->outputs[u].data(), c->outputs[u].size());
+            o = &c->joined[i];
+            o->clear();
+            if (zjoin[first[i]]) zlib0_join(parts, &member_adler[first[i]], *o);
+            else for (const auto& pc : parts) o->insert(o->end(), pc.first, pc.first + pc.second);
+        }
+        out[i].status = st;
+        out[i].data = st ? nullptr : o->data();
+        out[i].len = st ? 0 : o->size();
+    });
     return rc;
 }
 
@@ -922,6 +949,24 @@ int lepb200_host_lep_lazy_equal(const uint8_t* data, size_t len) {
     return 0;
 }
 int lepb200_host_brotli_available(void) { return brotli_available() ? 1 : 0; }
+int lepb200_host_lep_members(const uint8_t* data, size_t len, lepb200_lep_member* out, int cap) {
+    if (!data || (cap > 0 && !out)) return LEPB200_ERR_INVALID;
+    std::vector<std::unique_ptr<LepFile>> ms;
+    read_lep_members(data, len, ms, /*lazy=*/true);
+    for (size_t k = 0; k < ms.size() && (int)k < cap; ++k) out[k] = lepb200_lep_member{ms[k]->status, ms[k]->jpeg_size, ms[k]->nseg};
+    return (int)ms.size();
+}
+int lepb200_host_lep_open_member(const uint8_t* data, size_t len, int index, lepb200_lep** out, int32_t* status) {
+    if (!out || !data) return LEPB200_ERR_INVALID;
+    std::vector<std::unique_ptr<LepFile>> ms;
+    read_lep_members(data, len, ms, /*lazy=*/false);
+    if (index < 0 || index >= (int)ms.size()) return LEPB200_ERR_INVALID;
+    lepb200_lep* h = new lepb200_lep();
+    h->lf = std::move(*ms[index]);
+    *out = h;
+    if (status) *status = h->lf.status;
+    return LEPB200_OK;
+}
 int lepb200_host_lep_henc_image(lepb200_lep* h, lepb200_henc_image* out) {
     if (!h || h->lf.status || !out) return LEPB200_ERR_INVALID;
     GpuRecodeSetup gs;

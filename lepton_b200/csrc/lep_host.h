@@ -11,6 +11,7 @@
 #include "../../include/lepton_b200.h"
 #include <cstdint>
 #include <cstring>
+#include <memory>
 #include <string>
 #include <utility>
 #include <vector>
@@ -177,10 +178,19 @@ struct LepFile {
     // copy -- the batch decoder gathers them straight into its pinned staging buffer; `streams` then stays empty
     std::vector<std::vector<std::pair<const uint8_t*, uint32_t>>> spans;
     std::vector<size_t> stream_len;
+    size_t member_end = 0;           // bytes up to and including the mux's EOF marker; 0 without one (version 1)
     int status = OK;
     std::string error;
 };
-bool read_lep(const uint8_t* data, size_t n, LepFile& lf, bool lazy = false);
+// `carry` (member walk only): in, the header sections a -lepcat file's first member left for this one (the container's own
+// blob must then be empty); out, the sections behind this member's CNT marker.  Without it a CNT marker is unknown data.
+bool read_lep(const uint8_t* data, size_t n, LepFile& lf, bool lazy = false, std::vector<uint8_t>* carry = nullptr);
+// The members of a stream of concatenated .lep files (`cat a.lep b.lep`, -lepcat files; process_file, jpgcoder.cc:1867-1898):
+// every member read_lep gives, up to and including the first that fails.  The stream ends behind a member without an EOF
+// marker (version 1), or where fewer than 6 bytes follow the marker, or where the 2 bytes behind the size trailer are not
+// the first member's magic.  A progressive ('X') member behind a 'Z' one fails with ASSERTION_FAILURE, as the reference's
+// baseline re-encoder does on it.
+void read_lep_members(const uint8_t* data, size_t n, std::vector<std::unique_ptr<LepFile>>& out, bool lazy);
 bool brotli_available();          // libbrotlidec could be loaded: container versions 2 / 4 (brotli header blob) are read
 // Set-up for re-encoding the scan on the GPU (lepb200_huffman_encode_resident): false when the file needs the host
 // re-encoder (progressive, truncated, several scans, scan order != frame order, restart-marker budget).
@@ -200,11 +210,17 @@ void zlib0_frame(const uint8_t* data, size_t n, std::vector<uint8_t>& out);
 // JPEG bytes around a scan produced elsewhere: SOI + header up to the SOS + scan + trailing restart markers + rest of the
 // header + garbage (the tail of recode_baseline_jpeg, recoder.cc:839-886).  With JpegOut::zlib0_scan_adler, `scan_adler` is
 // the Adler-32 of the scan bytes and only the header and trailer bytes are summed here.
+// With `member_adler` (a member of a concatenated stream restored as one zlib stream) and a zlib0 mode, `out` gets the plain JPEG
+// and *member_adler its Adler-32, taken as the mode says; zlib0_join frames the members.
 bool assemble_baseline(const LepFile& lf, const GpuRecodeSetup& gs, const uint8_t* scan, std::vector<uint8_t>& out, std::string& err,
-                       JpegOut mode = JpegOut::plain, uint32_t scan_adler = 1);
+                       JpegOut mode = JpegOut::plain, uint32_t scan_adler = 1, uint32_t* member_adler = nullptr);
 // Re-create the JPEG bytes from decoded coefficient planes (recode_baseline_jpeg, src/lepton/recoder.cc:694-889).  A zlib0
 // output is recoded into a per-thread buffer first and framed from there (the host takes the whole Adler-32).
 bool recode_baseline(const LepFile& lf, const int16_t* const planes[4], std::vector<uint8_t>& out, std::string& err,
-                     JpegOut mode = JpegOut::plain);
+                     JpegOut mode = JpegOut::plain, uint32_t* member_adler = nullptr);
+// ONE zlib0 stream over the concatenated parts (the reference keeps one Zlib0Writer across the members of a stream,
+// bounded_iostream::prep_for_new_file): blocks of 65535 bytes run across part borders, and the Adler-32 is combined from
+// the parts' sums.
+void zlib0_join(const std::vector<std::pair<const uint8_t*, size_t>>& parts, const uint32_t* adlers, std::vector<uint8_t>& out);
 
 }  // namespace lephost

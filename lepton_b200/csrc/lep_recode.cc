@@ -74,7 +74,7 @@ int brotli_decompress(const uint8_t* in, size_t n, std::vector<uint8_t>& out, si
 
 bool brotli_available() { return brotli_api().ok; }
 
-bool read_lep(const uint8_t* d, size_t n, LepFile& lf, bool lazy) {
+bool read_lep(const uint8_t* d, size_t n, LepFile& lf, bool lazy, std::vector<uint8_t>* carry) {
     // CF 84 (tau): the usual container; CE B6 (zeta, zlepton_header, jpgcoder.cc:552): the same container whose JPEG is handed
     // out as a zlib stream (check_file, jpgcoder.cc:2200-2220)
     const bool zeta = n >= 2 && d[0] == 0xCE && d[1] == 0xB6;
@@ -90,7 +90,11 @@ bool read_lep(const uint8_t* d, size_t n, LepFile& lf, bool lazy) {
     if ((size_t)28 + zlen + 3 + 4 > n) return lfail(lf, SHORT_READ, "truncated .lep");
     // inflate the header blob
     std::vector<uint8_t> blob;
-    if (lf.version != 1) {
+    if (carry && !carry->empty()) {
+        // -lepcat: the first member's blob holds the headers of the members behind it, and theirs are empty (read_ujpg :4187-4189)
+        if (zlen != 0) return lfail(lf, ASSERTION_FAILURE, "Special concatenation requires 0 size header");
+        blob.swap(*carry);
+    } else if (lf.version != 1) {
         const int rc = brotli_decompress(d + 28, zlen, blob, size_t(256) << 20);
         if (rc == 1) return lfail(lf, NOT_HANDLED, "brotli header blob (container version 2 / 4) and no libbrotlidec on this system");
         if (rc == 3) return lfail(lf, 38 /*TOO_MUCH_MEMORY_NEEDED*/, "header blob too large");
@@ -119,6 +123,7 @@ bool read_lep(const uint8_t* d, size_t n, LepFile& lf, bool lazy) {
         if (ret != Z_STREAM_END) return lfail(lf, ASSERTION_FAILURE, "Data not properly zlib coded");
         blob.resize(have);
     }
+    if (carry) carry->clear();
     size_t p = 0;
     auto need = [&](size_t k) { return p + k <= blob.size(); };
     if (!need(7) || memcmp(&blob[p], "HDR", 3)) return lfail(lf, UNSUPPORTED_JPEG, "HDR marker not found");
@@ -206,6 +211,10 @@ bool read_lep(const uint8_t* d, size_t n, LepFile& lf, bool lazy) {
             if (!need(7 + (size_t)k)) return lfail(lf, SHORT_READ, "short PGE");
             j.prefix.assign(m + 7, m + 7 + k);
             p += 7 + (size_t)k;
+        } else if (carry && !memcmp(m, "CNT", 3)) {
+            // -lepcat: this member's sections end here; the rest of the blob belongs to the members behind it (:4328-4330)
+            carry->assign(m + 3, (const uint8_t*)blob.data() + blob.size());
+            break;
         } else if (!memcmp(m, "PGR", 3) || !memcmp(m, "SIZ", 3)) {
             return lfail(lf, NOT_HANDLED, "-startbyte slice sections (PGR / SIZ) are not handled");
         } else {
@@ -250,8 +259,9 @@ bool read_lep(const uint8_t* d, size_t n, LepFile& lf, bool lazy) {
     // demux (src/io/MuxReader.hh:230-283); the last 4 bytes are the file-size trailer
     if (lazy) { lf.spans.assign(16, {}); lf.stream_len.assign(16, 0); }
     else lf.streams.assign(16, std::vector<uint8_t>());
+    lf.member_end = 0;
     while (q + 3 <= end) {
-        if (d[q] == 0xFF && d[q + 1] == 0xFE && d[q + 2] == 0xFF) break;      // MuxReader::getEofMarker (MuxReader.hh:131-139,240-243), written by versions > 1
+        if (d[q] == 0xFF && d[q + 1] == 0xFE && d[q + 2] == 0xFF) { lf.member_end = q + 3; break; }   // MuxReader::getEofMarker (MuxReader.hh:131-139,240-243), written by versions > 1
         const uint8_t hd = d[q];
         const int sid = hd & 15, flags = (hd >> 4) & 3;
         size_t len, skip;
@@ -265,6 +275,29 @@ bool read_lep(const uint8_t* d, size_t n, LepFile& lf, bool lazy) {
     if (lazy) { lf.spans.resize(lf.nseg); lf.stream_len.resize(lf.nseg); }
     else lf.streams.resize(lf.nseg);
     return true;
+}
+
+void read_lep_members(const uint8_t* d, size_t n, std::vector<std::unique_ptr<LepFile>>& out, bool lazy) {
+    out.clear();
+    std::vector<uint8_t> carry;            // -lepcat: header sections of the members still to come
+    bool baseline_only = false;            // g_allow_progressive turned off by a member's flag (read_fixed_ujpg_header :2162-2166)
+    size_t o = 0;
+    for (;;) {
+        out.emplace_back(new LepFile());
+        LepFile& lf = *out.back();
+        if (!read_lep(d + o, n - o, lf, lazy, &carry)) return;
+        // A progressive member behind a 'Z' one is handed to the reference's baseline re-encoder, which asserts on it
+        // (recoder.cc:639, tests/golden/concat.json "baseline_then_progressive")
+        if (lf.flag == 'X' && baseline_only) { lfail(lf, ASSERTION_FAILURE, "progressive member behind a baseline one"); return; }
+        baseline_only |= lf.flag == 'Z' || (lf.flag & 1);
+        // version 1 has no EOF marker: the reference's mux reader takes everything up to the end of the stream
+        if (lf.member_end == 0) return;
+        // the 4-byte size trailer (not checked), then the magic of the next member: fewer than 6 bytes, or other magic
+        // bytes than the first member's, end the stream and the rest is ignored (process_file :1876-1896)
+        const size_t next = o + lf.member_end + 4;
+        if (next + 2 > n || d[next] != d[0] || d[next + 1] != d[1]) return;
+        o = next;
+    }
 }
 
 // ------------------------------------------------------------------------------------------------
@@ -431,8 +464,20 @@ void zlib0_frame(const uint8_t* data, size_t n, std::vector<uint8_t>& out) {
     w.finish((uint32_t)w.adler);
 }
 
+void zlib0_join(const std::vector<std::pair<const uint8_t*, size_t>>& parts, const uint32_t* adlers, std::vector<uint8_t>& out) {
+    size_t total = 0;
+    for (const auto& pc : parts) total += pc.second;
+    Zlib0Writer w(out, total, false);
+    uLong a = 1;
+    for (size_t k = 0; k < parts.size(); ++k) {
+        w.put(parts[k].first, parts[k].second);
+        a = adler32_combine(a, adlers[k], (z_off_t)parts[k].second);
+    }
+    w.finish((uint32_t)a);
+}
+
 bool assemble_baseline(const LepFile& lf, const GpuRecodeSetup& gs, const uint8_t* scan, std::vector<uint8_t>& out, std::string& err,
-                       JpegOut mode, uint32_t scan_adler) {
+                       JpegOut mode, uint32_t scan_adler, uint32_t* member_adler) {
     const Jpeg& j = lf.j;
     const std::vector<uint8_t>& h = j.hdr;
     static const uint8_t soi[2] = {0xFF, 0xD8};
@@ -449,10 +494,18 @@ bool assemble_baseline(const LepFile& lf, const GpuRecodeSetup& gs, const uint8_
     size_t total = 0;
     for (const auto& pc : pieces) total += pc.second;
     if (total != lf.jpeg_size) { err = "re-created JPEG has the wrong size"; out.clear(); return false; }
-    if (mode == JpegOut::plain) {
+    if (mode == JpegOut::plain || member_adler) {
         out.clear();
         out.reserve((size_t)lf.jpeg_size + 16);
         for (const auto& pc : pieces) out.insert(out.end(), pc.first, pc.first + pc.second);
+        if (!member_adler) return true;
+        if (mode == JpegOut::zlib0_host_adler) { *member_adler = (uint32_t)adler32(1, out.data(), (uInt)out.size()); return true; }
+        // the device's sum of the scan between the host's sums of the bytes in front of it and behind it
+        uLong head = 1, tail = 1;
+        size_t ntail = 0;
+        for (int k = 0; k < 3; ++k) head = adler32(head, pieces[k].first, (uInt)pieces[k].second);
+        for (int k = 4; k < 7; ++k) { tail = adler32(tail, pieces[k].first, (uInt)pieces[k].second); ntail += pieces[k].second; }
+        *member_adler = (uint32_t)adler32_combine(adler32_combine(head, scan_adler, (z_off_t)gs.scan_bytes), tail, (z_off_t)ntail);
         return true;
     }
     const bool host_sum = mode == JpegOut::zlib0_host_adler;
@@ -476,7 +529,13 @@ bool assemble_baseline(const LepFile& lf, const GpuRecodeSetup& gs, const uint8_
     return true;
 }
 
-bool recode_baseline(const LepFile& lf, const int16_t* const planes[4], std::vector<uint8_t>& out, std::string& err, JpegOut mode) {
+bool recode_baseline(const LepFile& lf, const int16_t* const planes[4], std::vector<uint8_t>& out, std::string& err, JpegOut mode,
+                     uint32_t* member_adler) {
+    if (mode != JpegOut::plain && member_adler) {
+        if (!recode_baseline(lf, planes, out, err, JpegOut::plain)) return false;
+        *member_adler = (uint32_t)adler32(1, out.data(), (uInt)out.size());
+        return true;
+    }
     if (mode != JpegOut::plain) {
         thread_local std::vector<uint8_t> jpeg;
         if (!recode_baseline(lf, planes, jpeg, err, JpegOut::plain)) { out.clear(); return false; }

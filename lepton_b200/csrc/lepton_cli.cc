@@ -16,6 +16,11 @@
 // -embedding=N: every input is a JPEG whose SOI sits at byte N of the file, whatever its first two bytes (check_file,
 // jpgcoder.cc:2192); the N bytes in front of it are kept in the .lep and come back in front of the JPEG on restore.
 // -d: the .lep keeps only the header segments the coefficients are coded with (rebuild_header_jpg, jpgcoder.cc:4848).
+// A .lep input may be a stream of concatenated .lep files (`cat a.lep b.lep | lepton-b200 -`, the reference's -lepcat files;
+// process_file, jpgcoder.cc:1867-1898): it is restored to the members' JPEGs one after the other, in single-file, stdin and
+// batch mode alike.  Writing -lepcat and -brotliheader files stays refused: both need brotli output identical to the
+// reference's vendored brotli 1.0.0, and the system's libbrotlienc 1.1.0 with the reference's BrotliCodec::Compress settings
+// gave other bytes in 40 of 81 compressions of this repository's files at quality 9-11.
 //
 // Batch mode (no reference counterpart; a GPU wants thousands of files per call, the reference one per process):
 //   lepton-b200 -outdir=DIR [-devices=0,1,...] a.jpg b.lep c.jpg ...
