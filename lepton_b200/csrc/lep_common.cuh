@@ -71,6 +71,49 @@ static_assert((M_EXPH % 16) == 0 && (M_HOT % 16) == 0 && (M_EXPX % 16) == 0 && (
 static_assert((M_NZ7T % 8) == 0 && (M_NZ7 % 8) == 0 && (M_NZE % 4) == 0, "count tree rows are read as 8- and 16-byte vectors");
 constexpr size_t MODEL_BYTES = size_t(M_TOTAL) * 2;
 
+// Interleaved model pool of the group decode kernel.  Segments of one batch hit largely the same contexts, but in a private
+// model a 32-byte sector that one segment touches holds 15 words it never uses.  The group kernel therefore stores the models
+// of MI_K consecutive jobs word pair by word pair: 4-byte unit u of model k of a block of W models sits at unit u * W + k,
+// so the words that the W segments share fill whole sectors, and the segments one warp decodes in lock step (consecutive
+// jobs) read the same sector when they are in the same state.  Every block holds W = MI_K models but the last one of a pool
+// of n jobs, which holds the n % MI_K that are left: the pool is exactly n models long, as with private models.
+// MI_K = 1 is the plain layout, one private model after the other.  Kernel A and the warp decode kernel keep private models.
+#ifndef LEPB200_MODEL_INTERLEAVE
+#define LEPB200_MODEL_INTERLEAVE 8
+#endif
+constexpr uint32_t MI_K = LEPB200_MODEL_INTERLEAVE;                  // models per interleave block
+constexpr uint32_t MI_UNIT = 2;                                      // words per unit (4 bytes)
+static_assert(MI_K >= 1 && (M_TOTAL % MI_UNIT) == 0, "a model is a whole number of units");
+// models in the block of job j, in a pool of n jobs (j < n)
+__host__ __device__ constexpr uint32_t mi_width(size_t j, size_t n) { return (uint32_t)(n - j / MI_K * MI_K < MI_K ? n - j / MI_K * MI_K : MI_K); }
+// u16 offset of word `word` of model k (k < width) inside its block of `width` models; offset(w, k) = offset(w, 0) + offset(0, k)
+__host__ __device__ constexpr uint32_t mi_offset(uint32_t word, uint32_t k, uint32_t width) {
+    return ((word / MI_UNIT) * width + k) * MI_UNIT + word % MI_UNIT;
+}
+// u16 offset of job j's model (its word 0) in a pool of n jobs, which is n * M_TOTAL words long
+__host__ __device__ constexpr size_t mi_model(size_t j, size_t n) {
+    return j / MI_K * MI_K * M_TOTAL + mi_offset(0, (uint32_t)(j % MI_K), mi_width(j, n));
+}
+// For every width W, mi_offset(., ., W) is a bijection of [0, M_TOTAL) x [0, W) onto [0, W * M_TOTAL): it writes
+// (word / MI_UNIT, k, word % MI_UNIT) in mixed radix (any, W, MI_UNIT).  Checked here on the first and last units of a block
+// of every width (tests/test_emu_model_interleave.py checks whole blocks and whole pools on the host).
+constexpr bool mi_round_trip(uint32_t width, uint32_t first, uint32_t n) {
+    for (uint32_t off = first; off < first + n; ++off) {
+        const uint32_t word = off / (MI_UNIT * width) * MI_UNIT + off % MI_UNIT, k = off / MI_UNIT % width;
+        if (word >= M_TOTAL || mi_offset(word, k, width) != off) return false;
+    }
+    return true;
+}
+constexpr bool mi_bijection() {
+    for (uint32_t w = 1; w <= MI_K; ++w)
+        if (!mi_round_trip(w, 0, 4 * w * MI_UNIT) || !mi_round_trip(w, w * M_TOTAL - 4 * w * MI_UNIT, 4 * w * MI_UNIT) ||
+            mi_offset(M_TOTAL - 1, w - 1, w) != w * M_TOTAL - 1)
+            return false;
+    return true;
+}
+static_assert(mi_bijection() && mi_model(MI_K, MI_K + 1) == (size_t)MI_K * M_TOTAL && mi_width(MI_K - 1, MI_K + 1) == MI_K &&
+              mi_width(MI_K, MI_K + 1) == 1, "interleave is a bijection");
+
 // 7x7 count tree: offset of row idx (2^(5-idx) words) in the tree's front part (idx >= 3) or rear part (idx < 3)
 __host__ __device__ constexpr uint32_t nz7_row(int idx) { return idx >= 3 ? 8u - (16u >> (idx - 2)) : 64u - (64u >> idx); }
 __host__ __device__ constexpr uint32_t m_nz7(int ci, int bin, int idx, int prefix) {
@@ -101,6 +144,11 @@ static_assert(m_exp_word(m_expdc(0, 0), 4) == M_EXPT && m_exp_next(m_exp_word(m_
               m_exp_word(m_expx(1, 7, 14, 11), 10) < M_NZ7, "exponent tails overlap");
 static_assert(m_nz7(1, 9, 0, 31) < M_NZE && m_nze(1, 1, 7, 7, 2, 3) < M_RESN && m_resn(1, 63, 9) + 15 < M_THR &&
               m_thr(1, 255, 7) + 127 < M_TOTAL, "model tables overlap");
+// every row the group kernel reads unit by unit starts on a unit: rows 2, 1, 0 of each 7x7 count tree, rows 1, 0 of each edge tree
+static_assert((m_nz7(0, 0, 0, 0) % MI_UNIT) == 0 && (m_nz7(0, 1, 0, 0) - m_nz7(0, 0, 0, 0)) % MI_UNIT == 0 &&
+              nz7_row(1) % MI_UNIT == 0 && nz7_row(2) % MI_UNIT == 0 && (m_nze(0, 0, 0, 0, 0, 0) % MI_UNIT) == 0 &&
+              (m_nze(0, 0, 0, 0, 1, 0) - m_nze(0, 0, 0, 0, 0, 0)) % MI_UNIT == 0 && (m_nze(0, 0, 0, 1, 0, 0) - m_nze(0, 0, 0, 0, 0, 0)) % MI_UNIT == 0,
+              "count tree rows start on a unit in every model of an interleave block");
 
 // ------------------------------------------------------------------------------------------------------
 // Small constant tables (reference: src/vp8/util/aligned_block.hh:32-55, src/vp8/model/jpeg_meta.hh:72-170 row 9).

@@ -14,9 +14,11 @@
 //   * the front region of the model (M_HOT words: signs, DC residuals, DC exponent heads, top rows of the 7x7 count
 //     trees) lives in shared memory, one copy per group, zero-filled when the group takes a
 //     segment.  A branch address below M_HOT selects the group's shared copy, any other the model in global memory,
-//     through a generic pointer, so the step loops keep one load per candidate and no branch.
+//     through a generic pointer, so the step loops keep one load per candidate and no branch;
+//   * the models of MI_K consecutive jobs are interleaved unit by unit (lep_common.cuh, mi_offset), and the groups of a warp
+//     claim their jobs together, so the segments of a warp share the sectors of the contexts they all use.
 //
-// Same job descriptors, model layout, work queue and results as lep_decode_group.cu.
+// Same job descriptors, work queue and results as lep_decode_group.cu.
 #include "lep_common.cuh"
 #include "lep_predict.cuh"
 
@@ -110,29 +112,41 @@ __device__ __forceinline__ uint32_t g2_half8(uint4 v, uint32_t i) {
 __device__ __forceinline__ uint32_t g2_half4(uint2 v, uint32_t i) {
     return (((i & 2u) ? v.y : v.x) >> ((i & 1u) << 4)) & 0xffffu;
 }
+// Global model words: `model` points at word 0 of the segment's model in the interleaved pool (lep_common.cuh, mi_model),
+// `width` is the number of models of its block, word `addr` is at model + mi_offset(addr, 0, width), and a unit (the word
+// pair addr, addr + 1 with addr even) is one 4-byte load.
+__device__ __forceinline__ uint16_t& g2_gword(uint16_t* model, uint32_t width, uint32_t addr) { return model[mi_offset(addr, 0, width)]; }
+__device__ __forceinline__ uint32_t g2_unit(const uint16_t* model, uint32_t width, uint32_t addr) {
+    return *reinterpret_cast<const uint32_t*>(model + mi_offset(addr, 0, width));
+}
+// 8 words from `addr` (even): four units
+__device__ __forceinline__ uint4 g2_units4(const uint16_t* model, uint32_t width, uint32_t addr) {
+    return make_uint4(g2_unit(model, width, addr), g2_unit(model, width, addr + 2), g2_unit(model, width, addr + 4),
+                      g2_unit(model, width, addr + 6));
+}
 // the 7x7 count tree (m_nz7): rows 5..2 hold 1, 2, 4, 8 words and do not depend on a bit of the count, so they are
 // requested together, as early as the tree is known: rows 5..3 from the front region in shared memory (`top` = row 3),
-// row 2 from the tree's rear part in global memory (`rear` = row 0)
+// row 2 from the tree's rear part in global memory (`rear` = address of row 0)
 struct G2NzTop { uint32_t r5, r4; uint2 r3; uint4 r2; };
-__device__ __forceinline__ G2NzTop g2_nz_top(const uint16_t* top, const uint16_t* rear) {
+__device__ __forceinline__ G2NzTop g2_nz_top(const uint16_t* top, const uint16_t* model, uint32_t width, uint32_t rear) {
     G2NzTop v;
     v.r5 = top[nz7_row(5) - nz7_row(3)];
     v.r4 = *reinterpret_cast<const uint32_t*>(top + (nz7_row(4) - nz7_row(3)));
     v.r3 = *reinterpret_cast<const uint2*>(top);
-    v.r2 = *reinterpret_cast<const uint4*>(rear + nz7_row(2));
+    v.r2 = g2_units4(model, width, rear + nz7_row(2));
     return v;
 }
 // the branch word at `addr`: the group's shared copy of the front region, or the segment's model in global memory
-__device__ __forceinline__ uint16_t* g2_word(uint16_t* hot, uint16_t* model, uint32_t addr) {
-    return (addr < M_HOT ? hot : model) + addr;
+__device__ __forceinline__ uint16_t* g2_word(uint16_t* hot, uint16_t* model, uint32_t width, uint32_t addr) {
+    return addr < M_HOT ? hot + addr : &g2_gword(model, width, addr);
 }
-// an edge count tree (m_nze): rows 2, 1, 0 of 1, 2, 4 words, 24 bytes in all
+// an edge count tree (m_nze) at address t: rows 2, 1, 0 of 1, 2, 4 words
 struct G2EdgeTree { uint32_t r2, r1; uint2 r0; };
-__device__ __forceinline__ G2EdgeTree g2_edge_tree(const uint16_t* t) {
+__device__ __forceinline__ G2EdgeTree g2_edge_tree(const uint16_t* model, uint32_t width, uint32_t t) {
     G2EdgeTree v;
-    v.r2 = t[2 << 2];
-    v.r1 = *reinterpret_cast<const uint32_t*>(t + (1 << 2));
-    v.r0 = *reinterpret_cast<const uint2*>(t);
+    v.r2 = model[mi_offset(t + (2 << 2), 0, width)];
+    v.r1 = g2_unit(model, width, t + (1 << 2));
+    v.r0 = make_uint2(g2_unit(model, width, t), g2_unit(model, width, t + 2));
     return v;
 }
 
@@ -231,6 +245,7 @@ lep_decode_g2_kernel(const ImageDesc* __restrict__ images, SegDesc* __restrict__
     SegDesc* sdp = nullptr;
     const ImageDesc* gp = images;
     uint16_t* model = model_pool;
+    uint32_t mwidth = 1;                  // models in the interleave block of `model`
     int seg_min_y = 0, seg_max_y = 0;
     bool seg_last = false;
     G2Bool br;
@@ -258,12 +273,17 @@ lep_decode_g2_kernel(const ImageDesc* __restrict__ images, SegDesc* __restrict__
 
     for (;;) {
         // ---- (0a) a free group takes the next segment of the queue
+        //      The groups of a warp that want one claim theirs together (one atomicAdd of their count), so the first wave gives
+        //      each warp S consecutive jobs from a multiple of S: at G = 4 exactly the MI_K models of one interleave block.
         const bool want_job = !alive && !exhausted;
-        if (__any_sync(FULL, want_job)) {
-            int job = -1;
-            if (want_job && sub == 0) job = atomicAdd(work_counter, 1);
-            job = __shfl_sync(FULL, job, gbase);
+        const unsigned claim = __ballot_sync(FULL, want_job && sub == 0);
+        if (claim) {
+            const int leader = __ffs(claim) - 1;
+            int job0 = 0;
+            if (lane == leader) job0 = atomicAdd(work_counter, __popc(claim));
+            job0 = __shfl_sync(FULL, job0, leader);
             if (want_job) {
+                const int job = job0 + __popc(claim & ((1u << gbase) - 1u));
                 if (job >= count) {
                     exhausted = true;
                 } else {
@@ -271,7 +291,8 @@ lep_decode_g2_kernel(const ImageDesc* __restrict__ images, SegDesc* __restrict__
                     sdp = &segs[sidx];
                     if (sdp->status == ST_OK) {               // else rejected on the host (e.g. zero quantiser, model.hh:257-262)
                         gp = &images[sdp->image];
-                        model = model_pool + (size_t)job * M_TOTAL;          // zero-filled before the launch
+                        model = model_pool + mi_model((size_t)job, (size_t)count);          // zero-filled before the launch
+                        mwidth = mi_width((size_t)job, (size_t)count);
                         seg_min_y = sdp->min_y; seg_max_y = sdp->max_y; seg_last = sdp->is_last != 0;
                         g2_init(br, reinterpret_cast<const uint8_t*>(sdp->stream), sdp->cap);
                         ndec = 0; top_mask = 7u; index = 0;
@@ -365,7 +386,7 @@ lep_decode_g2_kernel(const ImageDesc* __restrict__ images, SegDesc* __restrict__
                 else if (has_left && !has_above) ctx = (nz_left + 1) / 2;
                 else if (has_left && has_above) ctx = (nz_above + nz_left + 2) / 4;
                 cnt_top = m_nz7(ci, s_nzbin[ctx], 3, 0); cnt_rear = m_nz7(ci, s_nzbin[ctx], 0, 0);
-                nzt = g2_nz_top(hot + cnt_top, model + cnt_rear);
+                nzt = g2_nz_top(hot + cnt_top, model, mwidth, cnt_rear);
             }
         }
         cnt_ready = false;
@@ -386,12 +407,13 @@ lep_decode_g2_kernel(const ImageDesc* __restrict__ images, SegDesc* __restrict__
                 uint32_t split = 0, bit = 0;
                 if (alive) bit = g2_bit(br, s_rcp, mw, split);
                 const uint32_t p1 = (prefix << 1) | bit;
-                if (alive && idx == 5) r1 = *reinterpret_cast<const uint4*>(model + cnt_rear + nz7_row(1) + (p1 << 3));
-                if (alive && idx == 4) r0 = *reinterpret_cast<const uint4*>(model + cnt_rear + nz7_row(0) + (p1 << 3));
+                if (alive && idx == 5) r1 = g2_units4(model, mwidth, cnt_rear + nz7_row(1) + (p1 << 3));
+                if (alive && idx == 4) r0 = g2_units4(model, mwidth, cnt_rear + nz7_row(0) + (p1 << 3));
                 if (idx >= 4) G2_EMU_BARRIER();
                 if (alive) {
-                    uint16_t* const row = idx >= 3 ? hot + cnt_top + (nz7_row(idx) - nz7_row(3)) : model + cnt_rear + nz7_row(idx);
-                    row[prefix] = (uint16_t)g2_model_word(mw, bit);
+                    const uint16_t neww = (uint16_t)g2_model_word(mw, bit);
+                    if (idx >= 3) hot[cnt_top + (nz7_row(idx) - nz7_row(3)) + prefix] = neww;
+                    else g2_gword(model, mwidth, cnt_rear + nz7_row(idx) + prefix) = neww;
                     g2_update(br, split, bit);
                     prefix = p1;
                 }
@@ -420,7 +442,7 @@ lep_decode_g2_kernel(const ImageDesc* __restrict__ images, SegDesc* __restrict__
                 addr = eb + eoff[0];
                 a1 = addr + 1; a0 = eb + eoff[1];          // after the first exponent bit of position 0
             }
-            uint32_t mw = busy ? *g2_word(hot, model, addr) : 0u;
+            uint32_t mw = busy ? *g2_word(hot, model, mwidth, addr) : 0u;
             while (__any_sync(FULL, busy)) {
                 if (busy) {
                     // ---- on the chain
@@ -428,10 +450,10 @@ lep_decode_g2_kernel(const ImageDesc* __restrict__ images, SegDesc* __restrict__
                     const uint32_t bit = g2_bit(br, s_rcp, mw, split);
                     const uint32_t naddr = bit ? a1 : a0;
                     const bool nbusy = bit ? b1 : b0;
-                    uint32_t mwn = nbusy ? *g2_word(hot, model, naddr) : 0u;
+                    uint32_t mwn = nbusy ? *g2_word(hot, model, mwidth, naddr) : 0u;
                     // ---- in the shadow of that load: write-back, window, grammar state, decoded value
                     const uint32_t neww = g2_model_word(mw, bit);
-                    *g2_word(hot, model, addr) = (uint16_t)neww;   // all lanes of the group store the same value
+                    *g2_word(hot, model, mwidth, addr) = (uint16_t)neww;   // all lanes of the group store the same value
                     if (naddr == addr) mwn = neww;
                     g2_update(br, split, bit);
                     ++nd;
@@ -496,8 +518,8 @@ lep_decode_g2_kernel(const ImageDesc* __restrict__ images, SegDesc* __restrict__
         }
         G2EdgeTree eth = {}, etv = {};
         if (alive) {
-            eth = g2_edge_tree(model + m_nze(0, ci, eobx, (nz + 3) / 7, 0, 0));
-            etv = g2_edge_tree(model + m_nze(1, ci, eoby, (nz + 3) / 7, 0, 0));
+            eth = g2_edge_tree(model, mwidth, m_nze(0, ci, eobx, (nz + 3) / 7, 0, 0));
+            etv = g2_edge_tree(model, mwidth, m_nze(1, ci, eoby, (nz + 3) / 7, 0, 0));
             for (int k = sub; k < 14; k += G) {
                 int p = 0, coord;
                 if (k < 7) { coord = k + 1; if (has_above) p = lak_pred(rcur, rabove, icx + (k + 1) * 8, k + 1, 8); }
@@ -522,7 +544,7 @@ lep_decode_g2_kernel(const ImageDesc* __restrict__ images, SegDesc* __restrict__
                     uint32_t split = 0, bit = 0;
                     if (alive) {
                         bit = g2_bit(br, s_rcp, mw, split);
-                        model[base + ((uint32_t)idx << 2) + prefix] = (uint16_t)g2_model_word(mw, bit);
+                        g2_gword(model, mwidth, base + ((uint32_t)idx << 2) + prefix) = (uint16_t)g2_model_word(mw, bit);
                         g2_update(br, split, bit);
                         prefix = (prefix << 1) | bit;
                     }
@@ -545,7 +567,7 @@ lep_decode_g2_kernel(const ImageDesc* __restrict__ images, SegDesc* __restrict__
                 a1 = addr + 1;
                 a0 = expx_base + (uint32_t)ne * NE_STRIDE + POS_STRIDE + ((einfo[vert * 7 + 1] & 15u) << 2);
             }
-            uint32_t mw = busy ? *g2_word(hot, model, addr) : 0u;
+            uint32_t mw = busy ? *g2_word(hot, model, mwidth, addr) : 0u;
             while (__any_sync(FULL, busy)) {
                 if (busy) {
                     // ---- on the chain (see the 7x7 loop)
@@ -553,10 +575,10 @@ lep_decode_g2_kernel(const ImageDesc* __restrict__ images, SegDesc* __restrict__
                     const uint32_t bit = g2_bit(br, s_rcp, mw, split);
                     const uint32_t naddr = bit ? a1 : a0;
                     const bool nbusy = bit ? b1 : b0;
-                    uint32_t mwn = nbusy ? *g2_word(hot, model, naddr) : 0u;
+                    uint32_t mwn = nbusy ? *g2_word(hot, model, mwidth, naddr) : 0u;
                     // ---- in the shadow of that load
                     const uint32_t neww = g2_model_word(mw, bit);
-                    *g2_word(hot, model, addr) = (uint16_t)neww;
+                    *g2_word(hot, model, mwidth, addr) = (uint16_t)neww;
                     if (naddr == addr) mwn = neww;                 // saturated threshold index: the same branch twice in a row
                     g2_update(br, split, bit);
                     ++nd;
@@ -692,16 +714,16 @@ lep_decode_g2_kernel(const ImageDesc* __restrict__ images, SegDesc* __restrict__
             bool neg = false;
             uint32_t addr = dc_exp, a0 = dc_exp, a1 = dc_exp + 1;
             bool busy = alive, b0 = false, b1 = busy;
-            uint32_t mw = busy ? *g2_word(hot, model, addr) : 0u;
+            uint32_t mw = busy ? *g2_word(hot, model, mwidth, addr) : 0u;
             while (__any_sync(FULL, busy)) {
                 if (busy) {
                     uint32_t split;
                     const uint32_t bit = g2_bit(br, s_rcp, mw, split);
                     const uint32_t naddr = bit ? a1 : a0;
                     const bool nbusy = bit ? b1 : b0;
-                    uint32_t mwn = nbusy ? *g2_word(hot, model, naddr) : 0u;
+                    uint32_t mwn = nbusy ? *g2_word(hot, model, mwidth, naddr) : 0u;
                     const uint32_t neww = g2_model_word(mw, bit);
-                    *g2_word(hot, model, addr) = (uint16_t)neww;
+                    *g2_word(hot, model, mwidth, addr) = (uint16_t)neww;
                     if (naddr == addr) mwn = neww;
                     g2_update(br, split, bit);
                     ++nd;
@@ -778,7 +800,7 @@ lep_decode_g2_kernel(const ImageDesc* __restrict__ images, SegDesc* __restrict__
                 const int nza = has_above ? (int)rnz[x + 1] : 0;
                 const int bin = s_nzbin[has_above ? (nza + nz + 2) / 4 : (nz + 1) / 2];
                 cnt_top = m_nz7(ci, bin, 3, 0); cnt_rear = m_nz7(ci, bin, 0, 0);
-                nzt = g2_nz_top(hot + cnt_top, model + cnt_rear);
+                nzt = g2_nz_top(hot + cnt_top, model, mwidth, cnt_rear);
                 cnt_ready = true;
                 ++x; pc ^= 1; pa ^= 1;
             }
