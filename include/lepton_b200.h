@@ -110,6 +110,15 @@ int lepb200_encode_launch(lepb200_ctx* ctx);                                    
 int lepb200_encode_launch_symbolise(lepb200_ctx* ctx);
 int lepb200_encode_launch_rangecode(lepb200_ctx* ctx);
 int lepb200_encode_fetch(lepb200_ctx* ctx, lepb200_stream* out);                       /* sync + D2H streams */
+/* Test entry: an encode batch from caller token streams instead of kernel A, ready for lepb200_encode_launch_rangecode
+ * and lepb200_encode_fetch / lepb200_encode_fetch_files.  Segment s has ntok[s] tokens (probability | bit << 8; all
+ * segments back to back in `tokens`) and a stream slot of caps[s] bytes; the segments form nfiles files of seg_per_file[f]
+ * consecutive segments each.  The stream arena and the overflow arena of the batch are filled with canary bytes. */
+int lepb200_encode_upload_tokens(lepb200_ctx* ctx, const uint16_t* tokens, const uint32_t* ntok, const uint32_t* caps, int nseg,
+                                 const int32_t* seg_per_file, int nfiles);
+/* After the fetch of such a batch: moved[s] = 1 where stream s was placed in the overflow arena (it did not fit its slot),
+ * *changed = canary bytes overwritten behind the slots and behind the streams of the overflow arena. */
+int lepb200_encode_token_canaries(lepb200_ctx* ctx, uint8_t* moved, uint64_t* changed);
 int lepb200_decode_upload(lepb200_ctx* ctx, const lepb200_image* images, int nimages, const lepb200_stream* in);
 int lepb200_decode_launch(lepb200_ctx* ctx);
 int lepb200_decode_fetch(lepb200_ctx* ctx, const lepb200_image* images, int nimages, int32_t* status_out);
@@ -203,6 +212,9 @@ float lepb200_last_symbolise_ms(lepb200_ctx* ctx);
 float lepb200_last_huffman_ms(lepb200_ctx* ctx);
 /* Synchronisation iterations the sub-sequence Huffman kernels (lep_huffpar.cu) needed in that call; 0 = serial kernel only. */
 int lepb200_last_huffman_iterations(lepb200_ctx* ctx);
+/* Images of that call the sub-sequence kernels did not finish cleanly (an anomaly, or no convergence within the iteration
+ * budget), so that the serial kernel decoded them again from the start. */
+int lepb200_last_huffman_redone(lepb200_ctx* ctx);
 /* Number of kernel launches issued by this context so far (for bench.py's gpu_launches). */
 uint64_t lepb200_kernel_launches(const lepb200_ctx* ctx);
 /* Sum over the last uploaded batch of 128 * coded blocks + stream bytes (SURVEY.md section 8(d) algorithmic bytes);

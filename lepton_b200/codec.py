@@ -65,7 +65,7 @@ _EXPORTS = [
     "lepb200_host_lep_stream", "lepb200_host_lep_recode", "lepb200_host_lep_close", "lepb200_host_frontend_seconds",
     "lepb200_codec_set_zlib0", "lepb200_huffman_encode_adler32", "lepb200_host_lep_zlib0", "lepb200_host_zlib0_frame",
     "lepb200_codec_set_embedding", "lepb200_codec_set_discard_meta", "lepb200_host_jpeg_open_embedded",
-    "lepb200_host_lep_members", "lepb200_host_lep_open_member",
+    "lepb200_host_lep_members", "lepb200_host_lep_open_member", "lepb200_encode_upload_tokens", "lepb200_encode_token_canaries", "lepb200_last_huffman_redone",
 ]
 
 
@@ -283,6 +283,49 @@ class LeptonB200Codec:
         self.decode_upload(images, streams)
         self.decode_launch()
         return self.decode_fetch()
+
+    def range_code(self, streams, caps, files=None, headers=None):
+        """The range coder alone, on caller token streams (lepb200_encode_upload_tokens), launched and fetched as an encode
+        batch is: streams = uint16 token arrays (prob | bit << 8), caps = stream slot of each in bytes.
+        Without headers -> (per segment (status, bytes, moved to the overflow arena), changed canary bytes).
+        With files (segments per file, consecutive) and headers (per file everything in front of the mux packets) the
+        files are assembled on the device (lepb200_encode_fetch_files) -> (per file (status, bytes), moved, changed)."""
+        L = self._L
+        toks = [np.ascontiguousarray(t, dtype=np.uint16) for t in streams]
+        n = len(toks)
+        files = list(files) if files is not None else [1] * n
+        flat = np.concatenate(toks + [np.zeros(1, np.uint16)])
+        nt = (ctypes.c_uint32 * n)(*[len(t) for t in toks])
+        cp = (ctypes.c_uint32 * n)(*[int(c) for c in caps])
+        spf = (ctypes.c_int32 * len(files))(*files)
+        L.lepb200_encode_upload_tokens.argtypes = [ctypes.c_void_p, ctypes.c_void_p, ctypes.c_void_p, ctypes.c_void_p, ctypes.c_int,
+                                                   ctypes.c_void_p, ctypes.c_int]
+        L.lepb200_encode_launch_rangecode.argtypes = [ctypes.c_void_p]
+        L.lepb200_encode_token_canaries.argtypes = [ctypes.c_void_p, ctypes.c_void_p, ctypes.POINTER(ctypes.c_uint64)]
+        self._check(L.lepb200_encode_upload_tokens(self._ctx, flat.ctypes.data, nt, cp, n, spf, len(files)), "encode_upload_tokens")
+        self._check(L.lepb200_encode_launch_rangecode(self._ctx), "encode_launch_rangecode")
+        if headers is None:
+            out = (_Stream * n)()
+            self._check(L.lepb200_encode_fetch(self._ctx, out), "encode_fetch")
+            res = [(out[s].status, ctypes.string_at(out[s].data, out[s].len) if out[s].len else b"") for s in range(n)]
+        else:
+            if len(headers) != len(files):
+                raise LeptonB200Error("range_code: %d headers for %d files" % (len(headers), len(files)))
+            hb = [bytes(h) for h in headers]
+            bufs = (_Buffer * len(hb))()
+            for i, h in enumerate(hb):
+                bufs[i].data = ctypes.cast(ctypes.c_char_p(h), ctypes.c_void_p).value
+                bufs[i].len = len(h)
+            outf = (_Result * len(hb))()
+            L.lepb200_encode_fetch_files.argtypes = [ctypes.c_void_p, ctypes.POINTER(_Buffer), ctypes.POINTER(_Result)]
+            self._check(L.lepb200_encode_fetch_files(self._ctx, bufs, outf), "encode_fetch_files")
+            res = [(outf[i].status, ctypes.string_at(outf[i].data, outf[i].len) if outf[i].len else b"") for i in range(len(hb))]
+        moved = (ctypes.c_uint8 * n)()
+        bad = ctypes.c_uint64(0)
+        self._check(L.lepb200_encode_token_canaries(self._ctx, moved, ctypes.byref(bad)), "encode_token_canaries")
+        if headers is None:
+            return [(st, data, bool(moved[s])) for s, (st, data) in enumerate(res)], bad.value
+        return res, [bool(m) for m in moved], bad.value
 
     def sync(self):
         self._check(self._L.lepb200_sync(self._ctx), "sync")

@@ -104,6 +104,7 @@ struct lepb200_ctx {
     int huff_par = 1;                     // 1: images with enough entropy bytes take the many-threads-per-image kernels (lep_huffpar.cu)
     int huff_sub_bits = 0;                // bits per sub-sequence (one thread each); 0 = by batch size (LEPB200_HUFF_SUBSEQ_BITS overrides)
     int huff_par_iters = 0;               // synchronisation iterations of the last batch (diagnostic)
+    int huff_redone = 0;                  // images of the last batch the sub-sequence kernels left to the serial walk (diagnostic)
     int huff_warps = 4;                   // images per CTA of the Huffman kernel
     int host_threads = 1;                 // host threads this context may use for staging copies
     int rc_feed = -1;                     // range pass token feed: 1 = cp.async ring in shared memory, 0 = register ring of plain loads, -1 = by
@@ -124,7 +125,14 @@ struct lepb200_ctx {
     int dec_group_grid = 0;               // group kernel: CTAs of the current batch
     int dec_threads = 0;                  // group kernel: model slots of the current batch (0: the batch uses the warp kernel)
     bool stage_preuploaded = false;       // the caller pushed the staged scans itself (lepb200_huffman_stage_upload)
+    bool canary = false;                  // batch of lepb200_encode_upload_tokens: stream and overflow arenas hold canary bytes
+    size_t rc_ovf_used = 0;               // bytes of the overflow arena the last range coder run placed streams in
 };
+
+// lepb200_encode_upload_tokens / lepb200_encode_token_canaries: the byte the arenas are filled with, and how many of them
+// follow every stream slot and the streams of the overflow arena
+constexpr uint8_t CANARY_BYTE = 0xC3;
+constexpr size_t CANARY_BYTES = 256;
 
 #define CK(call)                                                                            \
     do {                                                                                    \
@@ -162,7 +170,7 @@ template <int G> void launch_group_kernel(int grid, cudaStream_t st, const Image
 
 // Common part of encode/decode upload: job tables (lep_plan.cuh), launch shape, pools, upload of the tables.
 int build_batch(lepb200_ctx* ctx, const lepb200_image* images, int nimages, bool encode, const lepb200_stream* in) {
-    ctx->have_batch = false; ctx->launched = false; ctx->is_encode = encode;
+    ctx->have_batch = false; ctx->launched = false; ctx->is_encode = encode; ctx->canary = false;
     BatchPlan& b = ctx->batch;
     if (const char* e = plan_batch(b, images, nimages, encode, in)) { ctx->err = e; return LEPB200_ERR_INVALID; }
     const int nseg = (int)b.segs.size();
@@ -218,6 +226,14 @@ __global__ void lep_compact_kernel(const SegDesc* __restrict__ segs, const unsig
     uint4* d4 = reinterpret_cast<uint4*>(dst);
     for (uint32_t i = threadIdx.x; i < n16; i += blockDim.x) d4[i] = s4[i];
     for (uint32_t i = n16 * 16 + threadIdx.x; i < n; i += blockDim.x) dst[i] = src[i];
+}
+
+// Overflow arena of the range coder for `used` bytes of streams; in a canary batch it is filled with canary bytes first.
+cudaError_t reserve_overflow(lepb200_ctx* ctx, size_t used) {
+    ctx->rc_ovf_used = used;
+    if (!ctx->canary) return ctx->d_rc_ovf.reserve(used);
+    const cudaError_t e = ctx->d_rc_ovf.reserve(used + CANARY_BYTES);
+    return e != cudaSuccess ? e : cudaMemsetAsync(ctx->d_rc_ovf.p, CANARY_BYTE, used + CANARY_BYTES, ctx->stream);
 }
 
 }  // namespace
@@ -329,6 +345,7 @@ float lepb200_last_symbolise_ms(lepb200_ctx* ctx) {
 }
 float lepb200_last_huffman_ms(lepb200_ctx* ctx) { return ctx ? ctx->last_ms_huff : -1.f; }
 int lepb200_last_huffman_iterations(lepb200_ctx* ctx) { return ctx ? ctx->huff_par_iters : 0; }
+int lepb200_last_huffman_redone(lepb200_ctx* ctx) { return ctx ? ctx->huff_redone : 0; }
 uint64_t lepb200_kernel_launches(const lepb200_ctx* ctx) { return ctx ? ctx->launches : 0; }
 uint64_t lepb200_last_algorithmic_bytes(const lepb200_ctx* ctx) { return ctx ? ctx->alg_bytes : 0; }
 
@@ -518,6 +535,8 @@ int lepb200_huffman_decode_to_device(lepb200_ctx* ctx, lepb200_jpeg_scan* scans,
     CK(cudaMemcpyAsync(hrows, ctx->d_hrows.p, rows_total, cudaMemcpyDeviceToHost, ctx->stream));
     CK(cudaStreamSynchronize(ctx->stream));
     cudaEventElapsedTime(&ctx->last_ms_huff, ctx->ev0, ctx->ev_mid);
+    ctx->huff_redone = 0;
+    for (int i = 0; i < n; ++i) ctx->huff_redone += hj[i].nsub != 0 && !(hj[i].par_done && !hj[i].par_redo);
     huffman_decode_results(scans, n, hj, hrows, d_rows);
     ctx->resident_plane_total = plane_total;
     ctx->resident_images = n;
@@ -565,6 +584,7 @@ int lepb200_encode_launch_rangecode(lepb200_ctx* ctx) {
     if (!ctx || !ctx->symbolised || !ctx->is_encode) { if (ctx) ctx->err = "encode_launch_rangecode without encode_launch_symbolise"; return LEPB200_ERR_INVALID; }
     CK(cudaSetDevice(ctx->device));
     const int nseg = (int)ctx->batch.segs.size();
+    ctx->rc_ovf_used = 0;
     if (ctx->rc_mode == 1) {
         // range-only pass -> digit layout (one small D2H + sync: the arena size depends on the data) -> parallel pieces -> carries
         SegDesc* ds = static_cast<SegDesc*>(ctx->d_segs.p);
@@ -587,7 +607,7 @@ int lepb200_encode_launch_rangecode(lepb200_ctx* ctx) {
         CK(cudaMemcpyAsync(totals, d_total, sizeof(totals), cudaMemcpyDeviceToHost, ctx->stream));
         CK(cudaStreamSynchronize(ctx->stream));
         const unsigned long long total_digits = totals[0];
-        if (totals[1]) CK(ctx->d_rc_ovf.reserve((size_t)totals[1]));
+        if (totals[1]) CK(reserve_overflow(ctx, (size_t)totals[1]));
         if (trace) cudaEventRecord(te[1], ctx->stream);
         CK(ctx->d_rc_digits.reserve((size_t)total_digits * 4 + 256));
         CK(cudaMemsetAsync(ctx->d_rc_digits.p, 0, (size_t)total_digits * 4, ctx->stream));
@@ -631,7 +651,7 @@ static int rerun_overflowed_serial(lepb200_ctx* ctx, SegDesc* hs, int nseg) {
     std::vector<int>& redo = ctx->rc_redo;
     const size_t total = plan_serial_rerun(hs, nseg, redo);
     if (redo.empty()) return LEPB200_OK;
-    CK(ctx->d_rc_ovf.reserve(total));
+    CK(reserve_overflow(ctx, total));
     CK(ctx->d_rc_redo.reserve(sizeof(int) * redo.size()));
     for (int s : redo) hs[s].stream += (unsigned long long)(uintptr_t)ctx->d_rc_ovf.p;
     const int n = (int)redo.size();
@@ -765,6 +785,90 @@ int lepb200_encode_images(lepb200_ctx* ctx, const lepb200_image* images, int nim
     r = lepb200_encode_launch(ctx);
     if (r) return r;
     return lepb200_encode_fetch(ctx, out);
+}
+
+// An encode batch as kernel A leaves it, from caller token streams: token slots as lep_token_offsets_kernel lays them out,
+// stream slots of caps[s] bytes each followed by CANARY_BYTES canary bytes, longest streams first.  Segments are grouped
+// into nfiles files (consecutive, seg_per_file[f] each) for lepb200_encode_fetch_files.
+int lepb200_encode_upload_tokens(lepb200_ctx* ctx, const uint16_t* tokens, const uint32_t* ntok, const uint32_t* caps, int nseg,
+                                 const int32_t* seg_per_file, int nfiles) {
+    if (!ctx || !tokens || !ntok || !caps || nseg <= 0 || !seg_per_file || nfiles <= 0) return LEPB200_ERR_INVALID;
+    CK(cudaSetDevice(ctx->device));
+    ctx->have_batch = ctx->launched = ctx->symbolised = false; ctx->is_encode = true; ctx->canary = true;
+    BatchPlan& b = ctx->batch;
+    b.images.assign(nfiles, ImageDesc());
+    b.segs.assign(nseg, SegDesc());
+    b.seg_blocks.assign(nseg, 0);
+    b.plane_bytes.assign((size_t)nfiles * 3, 0);
+    b.plane_total = b.stream_total = b.row_stride = 0;
+    b.tokens_known = true;
+    b.token_total = 0;
+    int s = 0;
+    for (int f = 0; f < nfiles; ++f) {
+        if (seg_per_file[f] < 1 || seg_per_file[f] > nseg - s) { ctx->err = "encode_upload_tokens: seg_per_file does not add up to nseg"; return LEPB200_ERR_INVALID; }
+        for (int k = 0; k < seg_per_file[f]; ++k, ++s) {
+            SegDesc& sd = b.segs[s];
+            sd.image = f;
+            sd.is_last = k + 1 == seg_per_file[f];
+            sd.ntok = ntok[s];
+            sd.tok_cap = token_slot(ntok[s]);
+            if (sd.ntok > sd.tok_cap) { ctx->err = "encode_upload_tokens: token stream too long"; return LEPB200_ERR_INVALID; }
+            sd.tokens = b.token_total;
+            b.token_total += sd.tok_cap;
+            sd.stream = b.stream_total;
+            sd.cap = caps[s];
+            b.stream_total += align_up((size_t)caps[s] + CANARY_BYTES, 256);
+        }
+    }
+    if (s != nseg) { ctx->err = "encode_upload_tokens: seg_per_file does not add up to nseg"; return LEPB200_ERR_INVALID; }
+    b.order.resize(nseg);
+    for (int i = 0; i < nseg; ++i) b.order[i] = i;
+    std::stable_sort(b.order.begin(), b.order.end(), [&](int x, int y) { return ntok[x] > ntok[y]; });
+    std::vector<uint16_t> tok((size_t)b.token_total, 0);
+    size_t src = 0;
+    for (int i = 0; i < nseg; ++i) { memcpy(tok.data() + b.segs[i].tokens, tokens + src, (size_t)ntok[i] * 2); src += ntok[i]; }
+    CK(ctx->d_streams.reserve(b.stream_total + 256));
+    CK(ctx->d_tokens.reserve((size_t)b.token_total * 2 + 256));
+    CK(ctx->d_images.reserve(sizeof(ImageDesc) * nfiles));
+    CK(ctx->d_segs.reserve(sizeof(SegDesc) * nseg));
+    CK(ctx->d_order.reserve(sizeof(int) * nseg));
+    CK(ctx->d_counter.reserve(256));
+    for (auto& sd : b.segs) sd.stream += (unsigned long long)(uintptr_t)ctx->d_streams.p;
+    CK(cudaMemsetAsync(ctx->d_streams.p, CANARY_BYTE, b.stream_total, ctx->stream));
+    CK(cudaMemcpyAsync(ctx->d_tokens.p, tok.data(), tok.size() * 2, cudaMemcpyHostToDevice, ctx->stream));
+    CK(cudaMemcpyAsync(ctx->d_images.p, b.images.data(), sizeof(ImageDesc) * nfiles, cudaMemcpyHostToDevice, ctx->stream));
+    CK(cudaMemcpyAsync(ctx->d_segs.p, b.segs.data(), sizeof(SegDesc) * nseg, cudaMemcpyHostToDevice, ctx->stream));
+    CK(cudaMemcpyAsync(ctx->d_order.p, b.order.data(), sizeof(int) * nseg, cudaMemcpyHostToDevice, ctx->stream));
+    CK(cudaEventRecord(ctx->ev0, ctx->stream));
+    CK(cudaEventRecord(ctx->ev_mid, ctx->stream));
+    CK(cudaStreamSynchronize(ctx->stream));
+    ctx->have_batch = ctx->symbolised = true;
+    return LEPB200_OK;
+}
+
+// After lepb200_encode_fetch(_files) of a lepb200_encode_upload_tokens batch: moved[s] = 1 where stream s ended up in the
+// overflow arena, *changed = canary bytes that are no longer canary bytes, behind every slot and behind the overflow arena.
+int lepb200_encode_token_canaries(lepb200_ctx* ctx, uint8_t* moved, uint64_t* changed) {
+    if (!ctx || !moved || !changed || !ctx->canary || !ctx->launched) { if (ctx) ctx->err = "encode_token_canaries without a fetched token batch"; return LEPB200_ERR_INVALID; }
+    CK(cudaSetDevice(ctx->device));
+    const BatchPlan& b = ctx->batch;
+    const int nseg = (int)b.segs.size();
+    std::vector<SegDesc> hs(nseg);
+    std::vector<uint8_t> arena(b.stream_total), tail(ctx->rc_ovf_used ? CANARY_BYTES : 0);
+    CK(cudaMemcpyAsync(hs.data(), ctx->d_segs.p, sizeof(SegDesc) * nseg, cudaMemcpyDeviceToHost, ctx->stream));
+    CK(cudaMemcpyAsync(arena.data(), ctx->d_streams.p, b.stream_total, cudaMemcpyDeviceToHost, ctx->stream));
+    if (!tail.empty()) CK(cudaMemcpyAsync(tail.data(), static_cast<uint8_t*>(ctx->d_rc_ovf.p) + ctx->rc_ovf_used, CANARY_BYTES, cudaMemcpyDeviceToHost, ctx->stream));
+    CK(cudaStreamSynchronize(ctx->stream));
+    const unsigned long long base = (unsigned long long)(uintptr_t)ctx->d_streams.p;
+    uint64_t bad = 0;
+    for (int s = 0; s < nseg; ++s) {
+        const size_t slot = (size_t)(b.segs[s].stream - base), end = slot + align_up((size_t)b.segs[s].cap + CANARY_BYTES, 256);
+        for (size_t k = slot + b.segs[s].cap; k < end; ++k) bad += arena[k] != CANARY_BYTE;
+        moved[s] = hs[s].stream < base || hs[s].stream >= base + b.stream_total;
+    }
+    for (uint8_t c : tail) bad += c != CANARY_BYTE;
+    *changed = bad;
+    return LEPB200_OK;
 }
 
 // ------------------------------------------------------------------------------------------------ GPU Huffman encode

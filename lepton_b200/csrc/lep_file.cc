@@ -389,7 +389,8 @@ int lepb200_compress_jpegs(lepb200_codec* c, const lepb200_buffer* jpegs, int n,
                 s.gpu_rc = lepb200_huffman_decode_to_device(ctx, s.scans.data(), nb);
                 c->t_huff_ms = lepb200_last_huffman_ms(ctx);
                 mark("huffman", k, t0);
-                if (trace) fprintf(stderr, "[trace]   huffman kernels %.1f ms, %d synchronisation iterations\n", c->t_huff_ms, lepb200_last_huffman_iterations(ctx));
+                if (trace) fprintf(stderr, "[trace]   huffman kernels %.1f ms, %d synchronisation iterations, %d images redone by the serial kernel\n",
+                                 c->t_huff_ms, lepb200_last_huffman_iterations(ctx), lepb200_last_huffman_redone(ctx));
             }
             double t1 = now_s();
             s.imgs.resize(nb);

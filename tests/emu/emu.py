@@ -64,8 +64,9 @@ def lib():
     return _LIB
 
 
-def decode_images(kernel, images, streams, grid_cap=0):
-    """Same contract as LeptonB200Codec.decode_images: decodes into images[i].planes, returns (status, ndecisions) per segment."""
+def decode_images(kernel, images, streams, grid_cap=0, reverse=False):
+    """Same contract as LeptonB200Codec.decode_images: decodes into images[i].planes, returns (status, ndecisions) per segment.
+    reverse runs CTAs and threads in reverse order."""
     from lepton_b200.codec import _Image, _Stream
     n = sum(im.nseg for im in images)
     arr = (_Stream * n)()
@@ -81,7 +82,7 @@ def decode_images(kernel, images, streams, grid_cap=0):
     cim = (_Image * len(images))(*[im.to_c() for im in images])
     st = (ctypes.c_int32 * n)()
     nd = (ctypes.c_uint64 * n)()
-    rc = lib().emu_decode_images(int(kernel), int(grid_cap), cim, len(images), arr, st, nd)
+    rc = lib().emu_decode_images(int(kernel), int(grid_cap), int(bool(reverse)), cim, len(images), arr, st, nd)
     if rc != 0:
         raise RuntimeError("emu_decode_images failed with %d" % rc)
     return list(st), list(nd)
@@ -90,9 +91,10 @@ def decode_images(kernel, images, streams, grid_cap=0):
 ENC_KERNEL_A = 0
 
 
-def encode_images(images, grid_cap=0, kernel=0, tok_caps=False):
+def encode_images(images, grid_cap=0, kernel=0, tok_caps=False, reverse=False):
     """Same contract as LeptonB200Codec.encode_images: per image a list of (status, bytes, ndecisions) per segment.
-    tok_caps=True: returns (that list, token bound of every segment as the count pre-pass sized it)."""
+    tok_caps=True: returns (that list, token bound of every segment as the count pre-pass sized it).  reverse runs the
+    CTAs and threads of every launch in reverse order."""
     from lepton_b200.codec import _Image, _Stream
     n = sum(im.nseg for im in images)
     cim = (_Image * len(images))(*[im.to_c() for im in images])
@@ -100,7 +102,7 @@ def encode_images(images, grid_cap=0, kernel=0, tok_caps=False):
     cap = sum(im.blocks() for im in images) * 128 + 8192 * n          # a stream holds < 1 byte per decision
     arena = (ctypes.c_uint8 * cap)()
     tc = (ctypes.c_uint32 * n)()
-    rc = lib().emu_encode_images(int(kernel), int(grid_cap), cim, len(images), out, arena, ctypes.c_size_t(cap), tc)
+    rc = lib().emu_encode_images(int(kernel), int(grid_cap), int(bool(reverse)), cim, len(images), out, arena, ctypes.c_size_t(cap), tc)
     if rc != 0:
         raise RuntimeError("emu_encode_images failed with %d" % rc)
     res, k = [], 0
@@ -161,14 +163,14 @@ class _Scan(ctypes.Structure):
 HUFF_SERIAL, HUFF_SUBSEQ = 0, 1
 
 
-def huffman_decode(mode, jpegs, sub_bits=4096, iter_cap=62, mutate=None):
+def huffman_decode(mode, jpegs, sub_bits=4096, iter_cap=62, mutate=None, reverse=False):
     """Huffman-decodes whole JPEG files with the emulated kernels.  mode HUFF_SERIAL: lep_huffdecode_kernel (one warp per
     image); HUFF_SUBSEQ: the sub-sequence kernels of lep_huffpar.cu, then lep_huffdecode_kernel for what they left.
     Returns (results, info): per file None when the host front end does not hand the file to the GPU decoder, else a dict
     with status, padbit, end_bitpos, rows [(bitpos, lastdc, mcu_y, tokens)], planes [ndarray(blocks, 64)], host_planes,
     and the scan's nbytes (de-stuffed), ncmp and rsti;
     info = (synchronisation iterations, images the serial kernel had to redo).  `mutate(i, bytearray)` may damage the
-    de-stuffed entropy bytes of file i before decoding."""
+    de-stuffed entropy bytes of file i before decoding.  reverse runs the CTAs and threads of every launch in reverse order."""
     from lepton_b200.codec import HostJpeg, lib as product_lib
     L = product_lib()
     L.lepb200_host_jpeg_scan.argtypes = [ctypes.c_void_p, ctypes.POINTER(_Scan)]
@@ -208,7 +210,7 @@ def huffman_decode(mode, jpegs, sub_bits=4096, iter_cap=62, mutate=None):
     info = (ctypes.c_int * 2)()
     f = lib().emu_huffman_decode
     f.restype = ctypes.c_int
-    rc = f(int(mode), int(sub_bits), int(iter_cap), arr, n, pp, info)
+    rc = f(int(mode), int(sub_bits), int(iter_cap), int(bool(reverse)), arr, n, pp, info)
     if rc != 0:
         raise RuntimeError("emu_huffman_decode failed with %d" % rc)
     for k, i in enumerate(idx):

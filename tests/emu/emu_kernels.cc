@@ -63,7 +63,8 @@ void group_shape(int G, int& warps, int& per_warp) {
 // kernel: 0 = lep_decode_kernel (warp per segment, persistent CTAs; `grid_cap` > 0 limits the CTAs so that warps take
 // several segments from the queue), 200 + G = lep_decode_g2_kernel<G> (G lanes per segment).  Decodes into images[i].planes (zeroed first,
 // like the device arena); per-segment status and decision counts come back like lepb200_decode_fetch reports them.
-extern "C" int emu_decode_images(int kernel, int grid_cap, const lepb200_image* images, int nimages, const lepb200_stream* in,
+// reverse = 1 runs the launch's CTAs and threads in reverse order (emu::g_reverse).
+extern "C" int emu_decode_images(int kernel, int grid_cap, int reverse, const lepb200_image* images, int nimages, const lepb200_stream* in,
                                  int32_t* status_out, uint64_t* ndecisions_out) {
     const int gl = kernel % 100;
     const bool group = kernel / 100 == 2 && (gl == 1 || gl == 2 || gl == 4 || gl == 8 || gl == 16 || gl == 32);
@@ -101,7 +102,9 @@ extern "C" int emu_decode_images(int kernel, int grid_cap, const lepb200_image* 
     std::vector<uint16_t> models(slots * M_TOTAL, kernel == 0 ? 0x5a5a : 0);       // thread / group kernels: zero fill before the launch; the warp kernel clears its own
     std::vector<uint8_t> rows((group ? group_slots : slots) * b.row_stride, 0);
     a.models = models.data(); a.rows = rows.data();
+    emu::g_reverse = reverse != 0;
     emu::launch(grid, block, kernel_body, &a);
+    emu::g_reverse = false;
     for (int i = 0; i < nimages; ++i)
         for (int c = 0; c < images[i].ncmp; ++c)
             memcpy(images[i].planes[c], reinterpret_cast<const void*>(b.images[i].plane[c]), b.plane_bytes[(size_t)i * 3 + c]);
@@ -179,12 +182,14 @@ void run_range_coder(int kernel, EncArgs& a, unsigned long long total_tokens, st
 // CTAs (persistent warps then take several segments each).  kernel: 0 = parallel range coder, 1 = serial range coder,
 // 2 = parallel range coder whose range pass feeds tokens through registers (LEPB200_RC_FEED=0).  tok_caps (optional,
 // sum(nseg) entries) receives the token bound of every segment (the count pre-pass's, or the caller's seg_token_bound).
-extern "C" int emu_encode_images(int kernel, int grid_cap, const lepb200_image* images, int nimages, lepb200_stream* out, uint8_t* arena, size_t arena_cap,
-                                 uint32_t* tok_caps) {
+// reverse = 1 runs the CTAs and threads of every launch in reverse order (emu::g_reverse).
+extern "C" int emu_encode_images(int kernel, int grid_cap, int reverse, const lepb200_image* images, int nimages, lepb200_stream* out, uint8_t* arena,
+                                 size_t arena_cap, uint32_t* tok_caps) {
     if (!out || !arena) return LEPB200_ERR_INVALID;
     BatchPlan b;
     if (plan_batch(b, images, nimages, true, nullptr)) return LEPB200_ERR_INVALID;
     const int nseg = (int)b.segs.size();
+    emu::g_reverse = reverse != 0;
     std::vector<uint8_t> pv, sv;
     uint8_t* pbase = host_arena(pv, b.plane_total, 0);
     uint8_t* sbase = host_arena(sv, b.stream_total, 0);
@@ -222,6 +227,7 @@ extern "C" int emu_encode_images(int kernel, int grid_cap, const lepb200_image* 
     // parallel range coder (lep_capi.cu: rc_mode 1; kernel 2 = register-ring token feed) or the serial one (kernel 1, rc_mode 0)
     std::vector<uint8_t> ovf;
     run_range_coder(kernel, a, total_tokens, ovf);
+    emu::g_reverse = false;
     if (tok_caps) for (int s = 0; s < nseg; ++s) tok_caps[s] = segs[s].tok_cap;
     size_t used = 0;
     for (int s = 0; s < nseg; ++s) {
@@ -310,7 +316,8 @@ extern "C" int emu_range_code(int kernel, int reverse, int nseg, const uint16_t*
 // ---- baseline Huffman decode: lep_huffdecode_kernel alone (mode 0) or the sub-sequence kernels of lep_huffpar.cu followed
 // by it (mode 1), on the jobs of plan_huffman_decode (lep_plan.cuh), without a staging buffer.
 // planes[3 * i + c] = host plane of component c of scan i (receives the decoded plane); scans[i] outputs are filled like the
-// device call fills them.  info[0] = synchronisation iterations, info[1] = images the serial kernel had to redo.
+// device call fills them.  info[0] = synchronisation iterations, info[1] = images the serial kernel had to redo.  reverse = 1
+// runs the CTAs and threads of every launch in reverse order (emu::g_reverse).
 namespace {
 struct HuffArgs { HuffJob* jobs; int n; const HuffTableDev* tabs; int ntabs; HpArrays a; int iter; int last_iter; unsigned int* dirty; int which; };
 void huff_body(void* p) {
@@ -322,9 +329,10 @@ void huff_body(void* p) {
 }
 }  // namespace
 
-extern "C" int emu_huffman_decode(int mode, int sub_bits, int iter_cap, lepb200_jpeg_scan* scans, int n, int16_t** planes, int* info) {
+extern "C" int emu_huffman_decode(int mode, int sub_bits, int iter_cap, int reverse, lepb200_jpeg_scan* scans, int n, int16_t** planes, int* info) {
     HuffDecodePlan p;
     if (plan_huffman_decode(p, scans, n, mode == 1, sub_bits, nullptr, 0)) return LEPB200_ERR_INVALID;
+    emu::g_reverse = reverse != 0;
     std::vector<HuffJob>& jobs = p.jobs;
     std::vector<uint8_t> hv, rv, pv;
     uint8_t* hbase = host_arena(hv, p.huff_total, 0);              // the scans with the zero bytes the kernels read past their ends
@@ -365,6 +373,7 @@ extern "C" int emu_huffman_decode(int mode, int sub_bits, int iter_cap, lepb200_
     for (int i = 0; i < n; ++i) if (jobs[i].nsub && !(jobs[i].par_done && !jobs[i].par_redo)) ++redo;
     h.which = 0;
     emu::launch((n + 3) / 4, 4 * 32, huff_body, &h);
+    emu::g_reverse = false;
     huffman_decode_results(scans, n, jobs.data(), rbase, (unsigned long long)(uintptr_t)rbase);
     for (int i = 0; i < n; ++i)
         for (int c = 0; c < std::min(jobs[i].ncmp, 3); ++c)

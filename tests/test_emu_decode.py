@@ -20,6 +20,7 @@ from helpers import (EXTREMES, coef_image_from_lep, extreme_leps, geometry_of, g
 
 KERNELS = [emu.KERNEL_WARP]
 GROUPS = [emu.KERNEL_G2(g) for g in (1, 2, 4, 8, 16, 32)]       # lep_decode_g2_kernel<G>; the library ships G = 4, 8, 32
+SCHEDULES = [False, True]                                       # reverse: CTAs and threads in reverse order
 
 
 @pytest.mark.parametrize("kernel", KERNELS + [emu.KERNEL_G2(4)])
@@ -36,20 +37,23 @@ def test_golden_files_decode_to_the_reference_planes(kernel):
 
 @pytest.mark.parametrize("kernel", KERNELS + [emu.KERNEL_G2(8)])
 def test_one_launch_with_more_segments_than_a_warp(kernel):
-    """All golden files in one batch: > 32 segments, so several warps and a partly filled last one."""
-    imgs, streams_all, want = [], [], []
-    for name in golden_leps():
-        lf = load_lep(name)
-        planes, streams = oracle_decode_planes(lf)
-        imgs.append(coef_image_from_lep(lf, [np.full_like(p, -3) for p in planes]))
-        streams_all.append(streams[:lf.nseg])
-        want.append(planes)
-    assert sum(im.nseg for im in imgs) > 32
-    st, _ = emu.decode_images(kernel, imgs, streams_all, grid_cap=3)      # warp kernel: 12 persistent warps share the queue
-    assert all(s == 0 for s in st), st
-    for name, img, planes in zip(golden_leps(), imgs, want):
-        for c in range(img.ncmp):
-            assert np.array_equal(img.planes[c], planes[c]), "%s component %d" % (name, c)
+    """All golden files in one batch: > 32 segments, so several warps and a partly filled last one.  Under both schedules
+    of the emulator (the threads of each CTA in order and in reverse order): this is the golden decode case that runs
+    reversed, the test above decodes the same files one launch each."""
+    for reverse in SCHEDULES:
+        imgs, streams_all, want = [], [], []
+        for name in golden_leps():
+            lf = load_lep(name)
+            planes, streams = oracle_decode_planes(lf)
+            imgs.append(coef_image_from_lep(lf, [np.full_like(p, -3) for p in planes]))
+            streams_all.append(streams[:lf.nseg])
+            want.append(planes)
+        assert sum(im.nseg for im in imgs) > 32
+        st, _ = emu.decode_images(kernel, imgs, streams_all, grid_cap=3, reverse=reverse)     # warp kernel: 12 persistent warps share the queue
+        assert all(s == 0 for s in st), st
+        for name, img, planes in zip(golden_leps(), imgs, want):
+            for c in range(img.ncmp):
+                assert np.array_equal(img.planes[c], planes[c]), "%s component %d reverse %s" % (name, c, reverse)
 
 
 @pytest.mark.parametrize("kernel", KERNELS + GROUPS)
@@ -82,7 +86,8 @@ def test_random_planes_oracle_streams_decode_back(kernel, cfg):
 
 def test_damaged_streams_end_the_same_way_in_all_kernels_and_the_oracle():
     """Truncated / bit-flipped streams: whatever comes out (status 7 for an impossible non-zero count, or garbage
-    coefficients), the two kernels and the oracle must agree on status, decision count and every stored block."""
+    coefficients), the two kernels under both schedules and the oracle must agree on status, decision count and every
+    stored block."""
     rng = np.random.default_rng(99)
     lf = load_lep("androidcrop_t2.lep")
     planes, streams = oracle_decode_planes(lf)
@@ -103,11 +108,12 @@ def test_damaged_streams_end_the_same_way_in_all_kernels_and_the_oracle():
             want_rc.append(rc)
         got = {}
         for kernel in KERNELS + [emu.KERNEL_G2(4), emu.KERNEL_G2(8), emu.KERNEL_G2(32)]:
-            img = coef_image_from_lep(lf, [np.full_like(p, 11) for p in planes])
-            st, nd = emu.decode_images(kernel, [img], [bad])
-            got[kernel] = (st, nd, [p.copy() for p in img.planes])
-        a = got[emu.KERNEL_WARP]
-        for b in (got[emu.KERNEL_G2(4)], got[emu.KERNEL_G2(8)], got[emu.KERNEL_G2(32)]):
+            for reverse in SCHEDULES:
+                img = coef_image_from_lep(lf, [np.full_like(p, 11) for p in planes])
+                st, nd = emu.decode_images(kernel, [img], [bad], reverse=reverse)
+                got[kernel, reverse] = (st, nd, [p.copy() for p in img.planes])
+        a = got[emu.KERNEL_WARP, False]
+        for b in (v for k, v in got.items() if k != (emu.KERNEL_WARP, False)):
             assert a[0] == b[0] == want_rc and a[1] == b[1]
             for c in range(len(planes)):
                 assert np.array_equal(a[2][c], b[2][c])

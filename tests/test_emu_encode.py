@@ -21,17 +21,20 @@ KERNELS = [0, 1, 2]
 @pytest.mark.parametrize("kernel", KERNELS)
 def test_golden_batch_encode_matches_reference_streams(kernel):
     """All committed reference-written .lep files in ONE batch, three persistent CTAs sharing the work queue: emulated GPU
-    streams == the reference's streams."""
+    streams == the reference's streams.  With the parallel range coder (kernel 0) also with the CTAs and threads of every
+    launch in reverse order: kernel A and its shared queue are the same for every range coder, whose forms
+    test_emu_rangecoder.py runs reversed on their own."""
     imgs, want = [], []
     for name in golden_leps():
         lf = load_lep(name)
         planes, streams = oracle_decode_planes(lf)
         imgs.append(coef_image_from_lep(lf, planes))
         want.append(streams[:lf.nseg])
-    got = emu.encode_images(imgs, grid_cap=3, kernel=kernel)
-    for name, g, w in zip(golden_leps(), got, want):
-        assert [x[0] for x in g] == [0] * len(w), name
-        assert [x[1] for x in g] == list(w), name
+    for reverse in (False, True) if kernel == 0 else (False,):
+        got = emu.encode_images(imgs, grid_cap=3, kernel=kernel, reverse=reverse)
+        for name, g, w in zip(golden_leps(), got, want):
+            assert [x[0] for x in g] == [0] * len(w), (name, reverse)
+            assert [x[1] for x in g] == list(w), (name, reverse)
 
 
 @pytest.mark.parametrize("cfg", [

@@ -39,20 +39,22 @@ def check_equal(a, b, name):
 
 @pytest.mark.parametrize("sub_bits", [256, 1024, 4096])
 def test_golden_jpegs_both_kernels_match_the_host_decoder(sub_bits):
+    """Both kernels, with the CTAs and threads of every launch in order and in reverse order."""
     jpegs = [open(os.path.join(GOLDEN, n), "rb").read() for n in GOLDEN_JPEGS]
-    ser, _ = emu.huffman_decode(emu.HUFF_SERIAL, jpegs)
-    par, (iters, redo) = emu.huffman_decode(emu.HUFF_SUBSEQ, jpegs, sub_bits=sub_bits)
-    taken = 0
-    for n, s, p in zip(GOLDEN_JPEGS, ser, par):
-        assert (s is None) == (p is None), n
-        if s is None:
-            continue
-        taken += 1
-        assert s["status"] == 0, n
-        for got, want in zip(s["planes"], s["host_planes"]):
-            assert np.array_equal(got, want), n
-        check_equal(p, s, n)
-    assert taken >= 6 and iters >= 2 and redo == 0
+    for reverse in (False, True):
+        ser, _ = emu.huffman_decode(emu.HUFF_SERIAL, jpegs, reverse=reverse)
+        par, (iters, redo) = emu.huffman_decode(emu.HUFF_SUBSEQ, jpegs, sub_bits=sub_bits, reverse=reverse)
+        taken = 0
+        for n, s, p in zip(GOLDEN_JPEGS, ser, par):
+            assert (s is None) == (p is None), n
+            if s is None:
+                continue
+            taken += 1
+            assert s["status"] == 0, n
+            for got, want in zip(s["planes"], s["host_planes"]):
+                assert np.array_equal(got, want), n
+            check_equal(p, s, n)
+        assert taken >= 6 and iters >= 2 and redo == 0
 
 
 @pytest.mark.parametrize("w,h,q,sub", [(640, 480, 85, 2), (333, 211, 95, 0), (1024, 96, 60, 1), (64, 64, 85, 2), (1920, 1080, 85, 2)])
@@ -71,7 +73,7 @@ def test_synthetic_jpegs_subsequence_kernels(w, h, q, sub):
 
 def test_damaged_scans_fall_back_to_the_serial_walk():
     """Bit flips, a cut-off tail and appended junk: whatever the sub-sequence kernels meet, the outcome (status and, for
-    status 0, every output) is the serial kernel's."""
+    status 0, every output) is the serial kernel's, under both schedules."""
     jpegs = [pil_jpeg(100 + k, 320, 240) for k in range(6)]
 
     def mutate(i, buf):
@@ -87,22 +89,24 @@ def test_damaged_scans_fall_back_to_the_serial_walk():
         elif i == 5:
             buf[-1] ^= 0x01
     ser, _ = emu.huffman_decode(emu.HUFF_SERIAL, jpegs, mutate=mutate)
-    par, (iters, redo) = emu.huffman_decode(emu.HUFF_SUBSEQ, jpegs, sub_bits=1024, mutate=mutate)
     assert ser[0]["status"] == 0
     assert any(s["status"] != 0 for s in ser[1:])
-    for k, (s, p) in enumerate(zip(ser, par)):
-        assert p["status"] == s["status"], k
-        if s["status"] == 0:
-            check_equal(p, s, "image %d" % k)
-    assert redo >= 1
+    for reverse in (False, True):
+        par, (iters, redo) = emu.huffman_decode(emu.HUFF_SUBSEQ, jpegs, sub_bits=1024, mutate=mutate, reverse=reverse)
+        for k, (s, p) in enumerate(zip(ser, par)):
+            assert p["status"] == s["status"], (k, reverse)
+            if s["status"] == 0:
+                check_equal(p, s, "image %d, reverse %s" % (k, reverse))
+        assert redo >= 1
 
 
 def test_no_convergence_within_the_budget_is_handed_to_the_serial_kernel():
     jpegs = [pil_jpeg(5, 640, 480)]
     ser, _ = emu.huffman_decode(emu.HUFF_SERIAL, jpegs)
-    par, (iters, redo) = emu.huffman_decode(emu.HUFF_SUBSEQ, jpegs, sub_bits=256, iter_cap=1)
-    assert redo == 1
-    check_equal(par[0], ser[0], "iteration budget 1")
+    for reverse in (False, True):
+        par, (iters, redo) = emu.huffman_decode(emu.HUFF_SUBSEQ, jpegs, sub_bits=256, iter_cap=1, reverse=reverse)
+        assert redo == 1
+        check_equal(par[0], ser[0], "iteration budget 1, reverse %s" % reverse)
 
 
 # ---- the way back: lep_huffencode_kernel (one warp per thread-segment) on the emulator

@@ -111,23 +111,30 @@ def batch(sizes, seed):
 
 
 def check(kernel, sizes, seed, grid_cap):
-    imgs, streams, want = batch(sizes, seed)
-    st, nd = emu.decode_images(kernel, imgs, streams, grid_cap=grid_cap)
-    assert all(s == 0 for s in st), st
-    assert nd == [n for _, ns in want for n in ns]
-    for img, (planes, _) in zip(imgs, want):
-        for c in range(img.ncmp):
-            assert np.array_equal(img.planes[c], planes[c])
+    """The batch decoded with the threads of each CTA in order and in reverse order."""
+    for reverse in (False, True):
+        imgs, streams, want = batch(sizes, seed)
+        st, nd = emu.decode_images(kernel, imgs, streams, grid_cap=grid_cap, reverse=reverse)
+        assert all(s == 0 for s in st), st
+        assert nd == [n for _, ns in want for n in ns]
+        for img, (planes, _) in zip(imgs, want):
+            for c in range(img.ncmp):
+                assert np.array_equal(img.planes[c], planes[c])
+
+
+# (segments per image, seed, CTA cap of the emulated launch); test_gpu_kernel_edges.py decodes the same batches on the device
+PARTIAL_BLOCK = ([3, 1, 5, 4], 5, 0)
+SECOND_CLAIMS = ([8, 2, 7, 1, 6, 3, 5, 4, 9], 11, 1)
 
 
 @pytest.mark.parametrize("lanes", [4, 8])
 def test_segment_count_not_a_multiple_of_the_block(lanes):
     """13 segments: one whole block of 8 models and a partial one of 5, in a pool of exactly 13 models."""
-    check(emu.KERNEL_G2(lanes), [3, 1, 5, 4], seed=5, grid_cap=0)
+    check(emu.KERNEL_G2(lanes), *PARTIAL_BLOCK)
 
 
 @pytest.mark.parametrize("lanes", [4, 8])
 def test_groups_take_second_jobs_at_any_place_in_a_block(lanes):
     """One CTA (32 groups at G = 4, 16 at G = 8) for 45 segments of different lengths: groups that finish early claim
     again, alone or a few at a time, so later jobs start anywhere in a block and share it with jobs of other warps."""
-    check(emu.KERNEL_G2(lanes), [8, 2, 7, 1, 6, 3, 5, 4, 9], seed=11, grid_cap=1)
+    check(emu.KERNEL_G2(lanes), *SECOND_CLAIMS)

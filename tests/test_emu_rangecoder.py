@@ -76,10 +76,12 @@ def carry_tokens(rng, runs, run_len):
     return tok(a[:, 0], a[:, 1])
 
 
-def check(kernel, reverse, streams, cap_delta=None, caps=None):
+def check(kernel, reverse, streams, cap_delta=None, caps=None, run=None):
     """Codes `streams` in one launch; every stream must come back with status 0 and the oracle's bytes, no canary byte
     may change, and a stream lies in its slot exactly when the form can know it fits (serial: len < cap; parallel:
-    L + 1 < cap, L = len without the stop-rule byte).  -> the oracle's streams."""
+    L + 1 < cap, L = len without the stop-rule byte).  run(streams, caps) -> (per segment (status, bytes, moved), changed
+    canary bytes) codes them instead of the emulator (the device tests pass the library's range coder).  -> the oracle's
+    streams."""
     ref = []
     for s in streams:
         before = oracle.bool_counts()["stop_zero"]
@@ -88,7 +90,7 @@ def check(kernel, reverse, streams, cap_delta=None, caps=None):
         ref.append((b, oracle.bool_counts()["stop_zero"] > before))
     if caps is None:
         caps = [max(1, len(b) + cap_delta) for b, _ in ref]
-    got, bad = emu.range_code(kernel, streams, caps, reverse=reverse)
+    got, bad = run(streams, caps) if run else emu.range_code(kernel, streams, caps, reverse=reverse)
     assert bad == 0, "%d canary bytes changed" % bad
     for k, ((st, data, moved), (want, stop), cap) in enumerate(zip(got, ref, caps)):
         assert st == 0, (k, st, len(want), cap)
@@ -98,42 +100,36 @@ def check(kernel, reverse, streams, cap_delta=None, caps=None):
     return [b for b, _ in ref]
 
 
-@pytest.mark.parametrize("reverse", SCHEDULES)
-@pytest.mark.parametrize("kernel", KERNELS)
-def test_token_counts_around_pieces_and_loads(kernel, reverse):
+# The cases: each codes its streams with `code(streams, cap_delta=..., caps=...)`, which is `check` bound to one kernel
+# and schedule of the emulator or to the library's range coder on the device (test_gpu_kernel_edges.py).
+def token_counts_around_pieces_and_loads(code):
     """0 tokens (marker and stop bits only), fewer than one 8-token load, 1024-token piece borders, 8 pieces."""
     rng = np.random.default_rng(11)
     counts = [0, 1, 7, 8, 9, 1023, 1024, 1025, 8 * 1024 - 1, 8 * 1024, 8 * 1024 + 1]
-    check(kernel, reverse, [random_tokens(rng, n) for n in counts], cap_delta=4096)
+    code([random_tokens(rng, n) for n in counts], cap_delta=4096)
 
 
-@pytest.mark.parametrize("reverse", SCHEDULES)
-@pytest.mark.parametrize("kernel", KERNELS)
-def test_full_token_domain(kernel, reverse):
+def full_token_domain(code):
     """Every (bit, prob) pair, prob 0 included, many times over, in random order and in long runs of each."""
     rng = np.random.default_rng(12)
     every = tok(np.arange(512) >> 8, np.arange(512) & 0xff)
     runs = np.repeat(every, 9)
-    check(kernel, reverse, [rng.permutation(np.tile(every, 20)), runs, runs[::-1].copy()], cap_delta=64)
+    code([rng.permutation(np.tile(every, 20)), runs, runs[::-1].copy()], cap_delta=64)
 
 
-@pytest.mark.parametrize("reverse", SCHEDULES)
-@pytest.mark.parametrize("kernel", KERNELS)
-def test_carries_across_pieces_and_digit_steps(kernel, reverse):
+def carries_across_pieces_and_digit_steps(code):
     """Carry walks of hundreds of bytes.  The longest walk runs back over a run of more than 3000 tokens (any 2048
     consecutive tokens hold a piece border), and walks of 64 bytes or more are longer than a 32-digit step of the carry
     pass."""
     rng = np.random.default_rng(13)
     oracle.bool_counts(reset=True)
     streams = [carry_tokens(rng, 3, 3000), carry_tokens(rng, 6, 1200), carry_tokens(rng, 20, 100)]
-    check(kernel, reverse, streams, cap_delta=64)
+    code(streams, cap_delta=64)
     c = oracle.bool_counts()
     assert c["walk_max"] >= 200 and c["walks_64"] >= 6, c
 
 
-@pytest.mark.parametrize("reverse", SCHEDULES)
-@pytest.mark.parametrize("kernel", KERNELS)
-def test_capacity_edges_and_stop_byte(kernel, reverse):
+def capacity_edges_and_stop_byte(code):
     """Slots of len - 1, len, len + 1 and len + 2 bytes for 60 streams, about an eighth of which end with the extra zero
     byte of the stop rule: the same bytes in every case, nothing written past a slot, the stream moved to the overflow
     arena exactly when it may not fit."""
@@ -141,13 +137,11 @@ def test_capacity_edges_and_stop_byte(kernel, reverse):
     streams = [random_tokens(rng, int(n)) for n in rng.integers(0, 3000, 60)]
     oracle.bool_counts(reset=True)
     for d in (-1, 0, 1, 2):
-        check(kernel, reverse, streams, cap_delta=d)
+        code(streams, cap_delta=d)
     assert oracle.bool_counts()["stop_zero"] >= 4 * 4
 
 
-@pytest.mark.parametrize("reverse", SCHEDULES)
-@pytest.mark.parametrize("kernel", KERNELS)
-def test_batch_of_mixed_segments(kernel, reverse):
+def batch_of_mixed_segments(code):
     """240 segments of mixed lengths and kinds in one launch (two CTAs of the range pass, 60 warps of the carry pass),
     slots from far too small to roomy."""
     rng = np.random.default_rng(15)
@@ -157,14 +151,56 @@ def test_batch_of_mixed_segments(kernel, reverse):
         streams.append(carry_tokens(rng, 2, 300) if k % 7 == 3 else random_tokens(rng, n))
     lens = [len(oracle.bool_encode(s)[1]) for s in streams]
     caps = [max(1, int(n * f)) for n, f in zip(lens, rng.choice([0.5, 0.99, 1.0, 1.01, 2.0], len(lens)))]
-    check(kernel, reverse, streams, caps=caps)
+    code(streams, caps=caps)
+
+
+def stream_of_more_than_a_million_tokens(code):
+    """More than 1024 pieces in one segment: the piece threads of the grid (8 CTAs x 128) stride over them."""
+    rng = np.random.default_rng(16)
+    s = np.concatenate([random_tokens(rng, 600000), carry_tokens(rng, 4, 4000), random_tokens(rng, 450001)])
+    assert len(s) > (1 << 20) and len(s) // 1024 > 8 * 128
+    code([s], cap_delta=-1000)
+
+
+CASES = [token_counts_around_pieces_and_loads, full_token_domain, carries_across_pieces_and_digit_steps,
+         capacity_edges_and_stop_byte, batch_of_mixed_segments, stream_of_more_than_a_million_tokens]
+
+
+def on_emulator(kernel, reverse):
+    return lambda streams, **kw: check(kernel, reverse, streams, **kw)
+
+
+@pytest.mark.parametrize("reverse", SCHEDULES)
+@pytest.mark.parametrize("kernel", KERNELS)
+def test_token_counts_around_pieces_and_loads(kernel, reverse):
+    token_counts_around_pieces_and_loads(on_emulator(kernel, reverse))
+
+
+@pytest.mark.parametrize("reverse", SCHEDULES)
+@pytest.mark.parametrize("kernel", KERNELS)
+def test_full_token_domain(kernel, reverse):
+    full_token_domain(on_emulator(kernel, reverse))
+
+
+@pytest.mark.parametrize("reverse", SCHEDULES)
+@pytest.mark.parametrize("kernel", KERNELS)
+def test_carries_across_pieces_and_digit_steps(kernel, reverse):
+    carries_across_pieces_and_digit_steps(on_emulator(kernel, reverse))
+
+
+@pytest.mark.parametrize("reverse", SCHEDULES)
+@pytest.mark.parametrize("kernel", KERNELS)
+def test_capacity_edges_and_stop_byte(kernel, reverse):
+    capacity_edges_and_stop_byte(on_emulator(kernel, reverse))
+
+
+@pytest.mark.parametrize("reverse", SCHEDULES)
+@pytest.mark.parametrize("kernel", KERNELS)
+def test_batch_of_mixed_segments(kernel, reverse):
+    batch_of_mixed_segments(on_emulator(kernel, reverse))
 
 
 @pytest.mark.slow
 @pytest.mark.parametrize("kernel", KERNELS)
 def test_stream_of_more_than_a_million_tokens(kernel):
-    """More than 1024 pieces in one segment: the piece threads of the grid (8 CTAs x 128) stride over them."""
-    rng = np.random.default_rng(16)
-    s = np.concatenate([random_tokens(rng, 600000), carry_tokens(rng, 4, 4000), random_tokens(rng, 450001)])
-    assert len(s) > (1 << 20) and len(s) // 1024 > 8 * 128
-    check(kernel, kernel == 0, [s], cap_delta=-1000)
+    stream_of_more_than_a_million_tokens(on_emulator(kernel, kernel == 0))

@@ -93,8 +93,11 @@ def test_extreme_batch_decode_matches_reference_planes(monkeypatch, mode, lanes)
     dict(gpu_huffman=True, env={"LEPB200_HUFF_PAR": "1", "LEPB200_HUFF_SUBSEQ_BITS": "512"}),
     dict(gpu_huffman=True, env={"LEPB200_DEVICE_MUX": "0"}),
     dict(gpu_huffman=True, env={"LEPB200_DEVICE_MUX": "1"}),
+    # 256-bit sub-sequences: the 16-bit codes of some files do not resynchronise within the 62 iterations, so the serial
+    # kernel redoes them on the device
+    dict(gpu_huffman=True, env={"LEPB200_HUFF_SUBSEQ_BITS": "256", "LEPB200_TRACE": "1"}, serial_redo=True),
 ])
-def test_extreme_files_compress_to_the_reference_lep_and_back(monkeypatch, cfg):
+def test_extreme_files_compress_to_the_reference_lep_and_back(monkeypatch, capfd, cfg):
     """File API: compress gives the reference CLI's .lep byte for byte (status 6 and no output for the refused files);
     decompress restores every input, the colour files through the device Huffman encoder when it is on."""
     from lepton_b200 import LeptonB200FileCodec
@@ -124,6 +127,10 @@ def test_extreme_files_compress_to_the_reference_lep_and_back(monkeypatch, cfg):
         assert md5(out) == EXTREMES[n]["back_md5"], n
     if cfg["gpu_huffman"]:
         assert recoded >= len(COLOUR), recoded
+    if cfg.get("serial_redo"):
+        import re
+        redone = [int(n) for n in re.findall(r"(\d+) images redone by the serial kernel", capfd.readouterr().err)]
+        assert redone and max(redone) > 0, redone        # files the sub-sequence kernels gave up on, decoded again serially
 
 
 @pytest.mark.parametrize("threads", [4, 8])
