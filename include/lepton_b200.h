@@ -299,6 +299,16 @@ void lepb200_codec_set_embedding(lepb200_codec* codec, long long offset);
  * coefficients are coded with (DQT, DHT, DRI, SOF0-2, SOS); APPn, COM and the rest are dropped, so the restored JPEG is
  * shorter than the input (with verification on, such a file fails with 41 as in the reference).  0 (default): all kept. */
 void lepb200_codec_set_discard_meta(lepb200_codec* codec, int on);
+/* -permissive (jpgcoder.cc:1111, validation.cc:25-218, generic_compress.cc:60-200): 1 = lepb200_compress_jpegs verifies every
+ * file (whatever lepb200_codec_set_verify says) and stores each one that ends with a non-zero status -- not a JPEG, damaged,
+ * arithmetic-coded, refused by the front end, failing verification (41), a .lep itself, inputs shorter than 2 bytes -- whole
+ * in the reference's generic container instead: flag 'Y', a fixed 1x1 grey JPEG header, the input in the PGE section, no
+ * coded streams.  Such a file gets status 0 and its container; only an empty input keeps a status (42, UNSUPPORTED_JPEG).
+ * The other files of the call take the device path and give the bytes they give without the setting.  With -embedding or
+ * -d the rule is the same, as in the reference: a -d file whose restore differs from the input fails verification and is
+ * stored generically.  lepb200_decompress_leps restores generic containers (plainly or as zlib0) from their PGE section,
+ * without device work; other 'Y' containers (-startbyte slices) stay refused with 200.  0 (default): off. */
+void lepb200_codec_set_permissive(lepb200_codec* codec, int on);
 /* device milliseconds of the last chunk's GPU Huffman-decode kernel (diagnostic) */
 double lepb200_codec_last_huffman_ms(const lepb200_codec* codec);
 /* files of the last lepb200_decompress_leps call whose scan was Huffman-encoded on the device (the rest went through the host re-encoder) */
@@ -386,6 +396,12 @@ int lepb200_host_lep_open_member(const uint8_t* data, size_t len, int index, lep
 /* test hook: the zlib stream lepb200_codec_set_zlib0 hands out for the `len` bytes at `data`.  Returns its length; writes it
  * to `out` only when cap is at least that length. */
 size_t lepb200_host_zlib0_frame(const uint8_t* data, size_t len, uint8_t* out, size_t cap);
+/* host halves of -permissive: the generic container lepb200_compress_jpegs writes for the `len` bytes at `data` (returns its
+ * length, 0 for an empty input; writes it to `out` only when cap is at least that length), and the bytes a generic container
+ * opened with lepb200_host_lep_open restores to, as zlib0 when `zlib0` is set or the file has the zeta magic
+ * (LEPB200_ERR_INVALID for any other container) */
+size_t lepb200_host_generic_lep(const uint8_t* data, size_t len, uint8_t* out, size_t cap);
+int lepb200_host_lep_generic(lepb200_lep* h, int zlib0, const uint8_t** data, size_t* len);
 /* diagnostic: wall-clock seconds of the host front end alone over a batch with `threads` workers */
 double lepb200_host_frontend_seconds(const lepb200_buffer* jpegs, int n, int threads, int32_t* first_error);
 

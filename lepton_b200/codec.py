@@ -66,6 +66,7 @@ _EXPORTS = [
     "lepb200_codec_set_zlib0", "lepb200_huffman_encode_adler32", "lepb200_host_lep_zlib0", "lepb200_host_zlib0_frame",
     "lepb200_codec_set_embedding", "lepb200_codec_set_discard_meta", "lepb200_host_jpeg_open_embedded",
     "lepb200_host_lep_members", "lepb200_host_lep_open_member", "lepb200_encode_upload_tokens", "lepb200_encode_token_canaries", "lepb200_last_huffman_redone",
+    "lepb200_codec_set_permissive", "lepb200_host_generic_lep", "lepb200_host_lep_generic",
 ]
 
 
@@ -402,6 +403,12 @@ def _bind_file_api(L):
     L.lepb200_codec_set_embedding.restype = None
     L.lepb200_codec_set_discard_meta.argtypes = [vp, ctypes.c_int]
     L.lepb200_codec_set_discard_meta.restype = None
+    L.lepb200_codec_set_permissive.argtypes = [vp, ctypes.c_int]
+    L.lepb200_codec_set_permissive.restype = None
+    L.lepb200_host_generic_lep.argtypes = [ctypes.c_char_p, ctypes.c_size_t, ctypes.c_void_p, ctypes.c_size_t]
+    L.lepb200_host_generic_lep.restype = ctypes.c_size_t
+    L.lepb200_host_lep_generic.argtypes = [vp, ctypes.c_int, ctypes.POINTER(vp), ctypes.POINTER(ctypes.c_size_t)]
+    L.lepb200_host_lep_generic.restype = ctypes.c_int
     L.lepb200_codec_set_even_split.argtypes = [vp, ctypes.c_int]
     L.lepb200_codec_set_even_split.restype = None
     L.lepb200_codec_set_verify.argtypes = [vp, ctypes.c_int]
@@ -552,6 +559,13 @@ class HostLep:
         """True for a container with the zeta magic (CE B6): its JPEG is restored as a zlib stream."""
         return bool(self._L.lepb200_host_lep_zlib0(self._h))
 
+    def restore_generic(self, zlib0: bool = False) -> bytes:
+        """The bytes a generic container of -permissive restores to (zlib0=True: as a zlib stream of stored blocks)."""
+        d, n = ctypes.c_void_p(), ctypes.c_size_t()
+        if self._L.lepb200_host_lep_generic(self._h, 1 if zlib0 else 0, ctypes.byref(d), ctypes.byref(n)) != 0:
+            raise LeptonB200Error("not a generic container (status %d: %s)" % (self.status, self.error))
+        return ctypes.string_at(d, n.value)
+
     def scan_layout(self):
         """(offset, length) of the entropy-coded scan in the original JPEG, (0, 0) if the host has to re-encode it."""
         off, n = ctypes.c_uint32(), ctypes.c_uint32()
@@ -605,6 +619,17 @@ def lep_members(data: bytes):
     return [(m.status, m.jpeg_size, m.nseg) for m in arr[:n]]
 
 
+def generic_lep(data: bytes) -> bytes:
+    """The generic container compress(..) writes with permissive=True for a file the coder cannot take (host code, no
+    GPU); b"" for an empty input, which has none."""
+    L = lib()
+    _bind_file_api(L)
+    n = L.lepb200_host_generic_lep(data, len(data), None, 0)
+    out = ctypes.create_string_buffer(max(n, 1))
+    assert L.lepb200_host_generic_lep(data, len(data), out, n) == n
+    return out.raw[:n]
+
+
 def zlib0_frame(data: bytes) -> bytes:
     """The zlib stream of stored blocks that decompress(..) hands out for these bytes with zlib0=True (host code, no GPU)."""
     L = lib()
@@ -619,12 +644,15 @@ class LeptonB200FileCodec:
     """JPEG bytes -> .lep bytes for a batch of files; host threads + one GPU.  zlib0=True (-zlib0): decompress hands every
     JPEG out as a zlib stream of stored blocks, as containers with the zeta magic (CE B6) always are.  embedding=N
     (-embedding=N): compress takes every input as a JPEG whose SOI sits at byte N, keeping the bytes in front of it in the
-    container.  discard_meta=True (-d): the container keeps only the header segments the coefficients are coded with."""
+    container.  discard_meta=True (-d): the container keeps only the header segments the coefficients are coded with.
+    permissive=True (-permissive): compress verifies every file and stores each one that would fail (whatever the reason,
+    inputs shorter than 2 bytes and non-JPEGs included) whole in the reference's generic container, restored byte for
+    byte by decompress; only an empty input keeps its status."""
 
     def __init__(self, device: int = 0, host_threads: int = 0, chunk_images: int = 0, gpu_huffman: bool = True,
                  allow_progressive: bool = True, min_encode_threads: int = 1, max_encode_threads: int = 8,
                  even_split: bool = False, verify: bool = False, zlib0: bool = False, embedding: Optional[int] = None,
-                 discard_meta: bool = False):
+                 discard_meta: bool = False, permissive: bool = False):
         self._L = lib()
         _bind_file_api(self._L)
         self._c = ctypes.c_void_p()
@@ -641,6 +669,7 @@ class LeptonB200FileCodec:
         self._L.lepb200_codec_set_zlib0(self._c, 1 if zlib0 else 0)                                # -zlib0
         self._L.lepb200_codec_set_embedding(self._c, -1 if embedding is None else embedding)         # -embedding=N
         self._L.lepb200_codec_set_discard_meta(self._c, 1 if discard_meta else 0)                  # -d
+        self._L.lepb200_codec_set_permissive(self._c, 1 if permissive else 0)                      # -permissive
 
     def close(self):
         if self._c:

@@ -19,6 +19,7 @@
 #include <vector>
 
 #include <cuda_runtime.h>
+#include <zlib.h>
 
 #include "../../include/lepton_b200.h"
 #include "lep_host.h"
@@ -44,6 +45,7 @@ struct lepb200_codec {
     bool zlib0 = false;            // -zlib0: restored JPEGs are handed out as zlib streams of stored blocks
     long long embedding = -1;      // -embedding=N (>= 0): every input is a JPEG whose SOI sits at byte N; the bytes in front are kept
     bool discard_meta = false;     // -d: the container keeps only the header segments the coefficients are coded with
+    bool permissive = false;       // -permissive: a file that fails (verification included) is stored in the generic container
     void* arena[4] = {nullptr, nullptr, nullptr, nullptr};  // pinned host memory for coefficient planes, one per in-flight chunk
     size_t arena_cap[4] = {0, 0, 0, 0};
     std::vector<std::vector<uint8_t>> outputs;
@@ -161,6 +163,7 @@ void lepb200_codec_set_verify(lepb200_codec* c, int on) { if (c) c->verify = on 
 void lepb200_codec_set_zlib0(lepb200_codec* c, int on) { if (c) c->zlib0 = on != 0; }
 void lepb200_codec_set_embedding(lepb200_codec* c, long long offset) { if (c) c->embedding = offset < 0 ? -1 : offset; }
 void lepb200_codec_set_discard_meta(lepb200_codec* c, int on) { if (c) c->discard_meta = on != 0; }
+void lepb200_codec_set_permissive(lepb200_codec* c, int on) { if (c) c->permissive = on != 0; }
 void lepb200_codec_set_encode_threads(lepb200_codec* c, int min_threads, int max_threads) {
     if (!c) return;
     c->min_encode_threads = (unsigned)std::min(std::max(min_threads, 1), 8);
@@ -528,8 +531,9 @@ int lepb200_compress_jpegs(lepb200_codec* c, const lepb200_buffer* jpegs, int n,
             for (int i = ranges[k].first; i < ranges[k].second; ++i) if (!status[i]) status[i] = 33;       // ExitCode::OS_ERROR
         }
     // -verify / -roundtrip (the reference CLI's default, jpgcoder.cc:1095-1110, validation.cc): every .lep is decoded
-    // again and must give back the input byte for byte; a file that does not is withheld with ROUNDTRIP_FAILURE (41)
-    if (c->verify && ret == LEPB200_OK) {
+    // again and must give back the input byte for byte; a file that does not is withheld with ROUNDTRIP_FAILURE (41).
+    // -permissive verifies every file whatever -verify says, as the reference does (jpgcoder.cc:1603)
+    if ((c->verify || c->permissive) && ret == LEPB200_OK) {
         std::vector<std::vector<uint8_t>> leps;
         leps.swap(c->outputs);
         std::vector<int> idx;
@@ -550,6 +554,21 @@ int lepb200_compress_jpegs(lepb200_codec* c, const lepb200_buffer* jpegs, int n,
             c->t_front += tf; c->t_gpu += tg; c->t_back += tb;                   // the verification pass is part of the call
         }
         c->outputs.swap(leps);
+    }
+    // -permissive (validation.cc:25-218, generic_compress.cc:60-200): every file that ended with a status, whichever,
+    // is stored whole in the generic container instead; only an empty one keeps a status (UNSUPPORTED_JPEG).  This is host
+    // work after the device path of the call, which ran as without the setting; the other files' bytes stay as they are.
+    if (c->permissive) {
+        std::vector<int> wrap;
+        for (int i = 0; i < n; ++i) if (status[i]) wrap.push_back(i);
+        const double t0 = now_s();
+        parallel_for((int)wrap.size(), c->nthreads, [&](int q) {
+            const int i = wrap[q];
+            std::string err;
+            if (write_generic_lep(jpegs[i].data, jpegs[i].len, c->outputs[i], err)) status[i] = 0;
+            else if (jpegs[i].len == 0) status[i] = UNSUPPORTED_JPEG;
+        });
+        c->t_back += now_s() - t0;
     }
     for (int i = 0; i < n; ++i) {
         if (status[i]) c->outputs[i].clear();
@@ -623,6 +642,25 @@ int lepb200_decompress_leps(lepb200_codec* c, const lepb200_buffer* leps, int n,
         if (pbytes[u] > c->plane_cap) { all[u]->status = NOT_HANDLED; all[u]->error = "image larger than the per-chunk device memory budget"; pbytes[u] = 0; }
     });
     std::vector<uint32_t> member_adler(nim, 1);       // zjoin images: Adler-32 of the restored member
+    // the images that take the device path (dev[k]: image of batch position k); the generic containers of -permissive are
+    // restored right here from their PGE section and take no gather, decode or re-encode work, so the batches, chunks and
+    // parts of the device re-encode of the other images are the same with them as without them
+    c->outputs.resize(nim);
+    for (auto& o : c->outputs) o.clear();
+    std::vector<int> dev;
+    dev.reserve(nim);
+    for (int u = 0; u < nim; ++u) if (!all[u]->generic) dev.push_back(u);
+    const int ndev = (int)dev.size();
+    if (ndev < nim) {
+        parallel_for(nim, c->nthreads, [&](int u) {
+            const LepFile& lf = *all[u];
+            if (!lf.generic) return;
+            const std::vector<uint8_t>& body = lf.j.prefix;
+            if (zjoin[u]) { c->outputs[u] = body; member_adler[u] = (uint32_t)adler32(1, body.data(), (uInt)body.size()); }
+            else if (c->zlib0 || lf.zlib0) zlib0_frame(body.data(), body.size(), c->outputs[u]);
+            else c->outputs[u] = body;
+        });
+    }
     c->t_front += now_s() - t_parse;
     mark("containers", -1, t_parse);
     // chunks of up to `plane_cap` bytes of coefficient planes (device memory: three contexts in flight).  The planes stay on the device
@@ -638,26 +676,24 @@ int lepb200_decompress_leps(lepb200_codec* c, const lepb200_buffer* leps, int n,
         // The two chunks in flight share the budget when a call does not fit in one.
         const size_t budget = c->gpu_huffman ? c->plane_cap : (size_t(6) << 30);
         size_t total = 0;
-        for (int i = 0; i < nim; ++i) total += pbytes[i];
+        for (int i = 0; i < ndev; ++i) total += pbytes[dev[i]];
         const size_t cap = total > budget ? budget / 2 : budget;
         const int chunk_max = std::max(1, c->chunk_images);
         int b0 = 0;
         size_t acc = 0;
-        for (int i = 0; i < nim; ++i) {
-            if (i > b0 && (i - b0 >= chunk_max || acc + pbytes[i] > cap)) { ranges.emplace_back(b0, i); b0 = i; acc = 0; }
-            acc += pbytes[i];
+        for (int i = 0; i < ndev; ++i) {
+            if (i > b0 && (i - b0 >= chunk_max || acc + pbytes[dev[i]] > cap)) { ranges.emplace_back(b0, i); b0 = i; acc = 0; }
+            acc += pbytes[dev[i]];
         }
-        ranges.emplace_back(b0, nim);
+        ranges.emplace_back(b0, ndev);
         W = std::max(1, std::min(std::min(2, c->concurrent), (int)ranges.size()));
     }
     keep_arenas_for(c, 2, W);
     const int pth = std::max(1, c->nthreads / W);
     const int nchunks = (int)ranges.size();
     // the output buffers keep their capacity from call to call (a fresh 1.5 GB of vectors per 4096-file call is 370 K
-    // page faults inside the container stage); every image's buffer is rewritten or cleared below.  Indices from here on
-    // are images (members), not inputs.
-    c->outputs.resize(nim);
-    for (auto& o : c->outputs) o.clear();
+    // page faults inside the container stage); every image's buffer was cleared above.  Chunks range over batch positions
+    // (dev), every other index from here on is an image (member), not an input.
     std::vector<int> status(nim, 0);
     struct DChunk {
         int begin = 0, end = 0;
@@ -684,8 +720,8 @@ int lepb200_decompress_leps(lepb200_codec* c, const lepb200_buffer* leps, int n,
         const int m = s.end - s.begin;
         s.lf.resize(m); s.planes.resize(m);
         for (int i = 0; i < m; ++i) {
-            s.lf[i] = std::move(all[s.begin + i]);
-            status[s.begin + i] = s.lf[i]->status;
+            s.lf[i] = std::move(all[dev[s.begin + i]]);
+            status[dev[s.begin + i]] = s.lf[i]->status;
             for (int q = 0; q < 4; ++q) s.planes[i][q] = nullptr;
             if (s.lf[i]->status == 0) s.idx.push_back(i);
         }
@@ -703,7 +739,7 @@ int lepb200_decompress_leps(lepb200_codec* c, const lepb200_buffer* leps, int n,
         // pinned arena for the planes of the files the host re-encodes
         size_t total = 0;
         std::vector<size_t> base(nb, 0);
-        for (int q = 0; q < nb; ++q) if (s.henc[q].scan_bytes == 0) { base[q] = total; total += pbytes[s.begin + s.idx[q]]; }
+        for (int q = 0; q < nb; ++q) if (s.henc[q].scan_bytes == 0) { base[q] = total; total += pbytes[dev[s.begin + s.idx[q]]]; }
         uint8_t* arena = nullptr;
         if (total) {
             if (!reserve_arena(c, k % W, total + 256)) { s.gpu_rc = LEPB200_ERR_NOMEM; return; }
@@ -767,7 +803,7 @@ int lepb200_decompress_leps(lepb200_codec* c, const lepb200_buffer* leps, int n,
     };
     // JPEG of one batch image from the scan the device produced
     auto assemble = [&](DChunk& s, int q, uint32_t scan_adler) {
-        const int li = s.idx[q], i = s.begin + li;
+        const int li = s.idx[q], i = dev[s.begin + li];
         for (int t = s.seg_base[q]; t < s.seg_base[q + 1]; ++t)
             if (s.seg_status[t]) { status[i] = s.seg_status[t]; return; }
         std::string err;
@@ -832,7 +868,7 @@ int lepb200_decompress_leps(lepb200_codec* c, const lepb200_buffer* leps, int n,
         if (s.gpu_rc == 0) {
             parallel_for(nb, pth, [&](int q) {
                 if (done[q]) return;
-                const int li = s.idx[q], i = s.begin + li;
+                const int li = s.idx[q], i = dev[s.begin + li];
                 for (int t = s.seg_base[q]; t < s.seg_base[q + 1]; ++t)
                     if (s.seg_status[t]) { status[i] = s.seg_status[t]; return; }
                 std::string err;
@@ -859,7 +895,7 @@ int lepb200_decompress_leps(lepb200_codec* c, const lepb200_buffer* leps, int n,
     for (int k = 0; k < nchunks; ++k)
         if (cs[k].gpu_rc) {
             rc = cs[k].gpu_rc; c->err = lepb200_last_error(c->ctx2[k % W]);
-            for (int i = ranges[k].first; i < ranges[k].second; ++i) if (!status[i]) status[i] = 33;       // ExitCode::OS_ERROR
+            for (int i = ranges[k].first; i < ranges[k].second; ++i) if (!status[dev[i]]) status[dev[i]] = 33;       // ExitCode::OS_ERROR
         }
     // back to inputs: the status of the first member that failed, else the members' JPEGs one after the other (one zlib
     // stream over all of them for zlib0 output).  A single member's buffer is handed out as it is.
@@ -899,19 +935,19 @@ int lepb200_host_lep_open(const uint8_t* data, size_t len, lepb200_lep** out, in
 const char* lepb200_host_lep_error(const lepb200_lep* h) { return h ? h->lf.error.c_str() : "null"; }
 // geometry + splits (planes pointers are left null: the caller provides the planes)
 int lepb200_host_lep_image(lepb200_lep* h, lepb200_image* img) {
-    if (!h || !img || h->lf.status) return LEPB200_ERR_INVALID;
+    if (!h || !img || h->lf.status || h->lf.generic) return LEPB200_ERR_INVALID;
     int16_t* none[4] = {nullptr, nullptr, nullptr, nullptr};
     fill_image(*img, h->lf.j, none, h->lf.handoffs);
     return LEPB200_OK;
 }
 int lepb200_host_lep_stream(lepb200_lep* h, int seg, const uint8_t** data, size_t* len) {
-    if (!h || h->lf.status || seg < 0 || seg >= h->lf.nseg) return LEPB200_ERR_INVALID;
+    if (!h || h->lf.status || h->lf.generic || seg < 0 || seg >= h->lf.nseg) return LEPB200_ERR_INVALID;
     *data = h->lf.streams[seg].data();
     *len = h->lf.streams[seg].size();
     return LEPB200_OK;
 }
 int lepb200_host_lep_recode(lepb200_lep* h, const int16_t* const planes[3], const uint8_t** data, size_t* len) {
-    if (!h || h->lf.status) return LEPB200_ERR_INVALID;
+    if (!h || h->lf.status || h->lf.generic) return LEPB200_ERR_INVALID;
     const int16_t* p4[4] = {planes[0], planes[1], planes[2], nullptr};
     std::string err;
     if (!recode_baseline(h->lf, p4, h->out, err)) { h->lf.error = err; return LEPB200_ERR_INVALID; }
@@ -922,7 +958,7 @@ int lepb200_host_lep_recode(lepb200_lep* h, const int16_t* const planes[3], cons
 // Host half of the device re-encode path: where the scan lies in the original file (0 = the file needs the host
 // re-encoder) and the assembly of the JPEG around scan bytes produced elsewhere.
 int lepb200_host_lep_scan_layout(lepb200_lep* h, uint32_t* scan_offset, uint32_t* scan_bytes) {
-    if (!h || h->lf.status || !scan_offset || !scan_bytes) return LEPB200_ERR_INVALID;
+    if (!h || h->lf.status || h->lf.generic || !scan_offset || !scan_bytes) return LEPB200_ERR_INVALID;
     GpuRecodeSetup gs;
     if (!gpu_recode_setup(h->lf, gs)) { *scan_offset = 0; *scan_bytes = 0; return LEPB200_OK; }
     *scan_offset = (uint32_t)(h->lf.j.prefix.size() + 2 + gs.hpos);
@@ -969,13 +1005,13 @@ int lepb200_host_lep_open_member(const uint8_t* data, size_t len, int index, lep
     return LEPB200_OK;
 }
 int lepb200_host_lep_henc_image(lepb200_lep* h, lepb200_henc_image* out) {
-    if (!h || h->lf.status || !out) return LEPB200_ERR_INVALID;
+    if (!h || h->lf.status || h->lf.generic || !out) return LEPB200_ERR_INVALID;
     GpuRecodeSetup gs;
     fill_henc_image(h->lf, gs, *out);
     return LEPB200_OK;
 }
 int lepb200_host_lep_assemble(lepb200_lep* h, const uint8_t* scan, size_t scan_len, const uint8_t** data, size_t* len) {
-    if (!h || h->lf.status || !scan) return LEPB200_ERR_INVALID;
+    if (!h || h->lf.status || h->lf.generic || !scan) return LEPB200_ERR_INVALID;
     GpuRecodeSetup gs;
     if (!gpu_recode_setup(h->lf, gs) || gs.scan_bytes != scan_len) return LEPB200_ERR_INVALID;
     std::string err;
@@ -985,6 +1021,23 @@ int lepb200_host_lep_assemble(lepb200_lep* h, const uint8_t* scan, size_t scan_l
     return LEPB200_OK;
 }
 void lepb200_host_lep_close(lepb200_lep* h) { delete h; }
+int lepb200_host_lep_generic(lepb200_lep* h, int zlib0, const uint8_t** data, size_t* len) {
+    if (!h || h->lf.status || !h->lf.generic || !data || !len) return LEPB200_ERR_INVALID;
+    const std::vector<uint8_t>& body = h->lf.j.prefix;
+    if (zlib0 || h->lf.zlib0) zlib0_frame(body.data(), body.size(), h->out);
+    else h->out = body;
+    *data = h->out.data();
+    *len = h->out.size();
+    return LEPB200_OK;
+}
+size_t lepb200_host_generic_lep(const uint8_t* data, size_t len, uint8_t* out, size_t cap) {
+    if (!data && len) return 0;
+    std::vector<uint8_t> lep;
+    std::string err;
+    if (!write_generic_lep(data, len, lep, err)) return 0;
+    if (out && cap >= lep.size()) memcpy(out, lep.data(), lep.size());
+    return lep.size();
+}
 int lepb200_host_lep_zlib0(const lepb200_lep* h) { return h && h->lf.zlib0 ? 1 : 0; }
 size_t lepb200_host_zlib0_frame(const uint8_t* data, size_t len, uint8_t* out, size_t cap) {
     if (!data && len) return 0;

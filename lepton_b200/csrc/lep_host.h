@@ -161,6 +161,13 @@ bool build_lep_header(const Jpeg& j, const Splits& sp, std::vector<uint8_t>& out
 bool write_lep(const Jpeg& j, const Splits& sp, const std::vector<std::pair<const uint8_t*, size_t>>& streams,
                std::vector<uint8_t>& out, std::string& err);
 
+// The generic container of -permissive (generic_compress.cc:60-200), for files the coder cannot take: flag 'Y', a fixed
+// 1x1 grey JPEG header, GENERIC_SEGMENTS zeroed handoffs, the whole input in the PGE section, an empty GRB section and no
+// coded streams.  Restoring it gives the input back byte for byte.  An empty input has none (false).
+enum { GENERIC_SEGMENTS = 8 };                   // the reference's MAX_NUM_THREADS, whatever -maxencodethreads says
+const std::vector<uint8_t>& generic_jpeg_header();   // the HDR section of every generic container
+bool write_generic_lep(const uint8_t* data, size_t n, std::vector<uint8_t>& out, std::string& err);
+
 // ---- decode side --------------------------------------------------------------------------------------
 struct LepFile {
     uint8_t version = 0, flag = 0;
@@ -172,6 +179,7 @@ struct LepFile {
     bool rst_cnt_set = false;        // CRS section present (jpgcoder.cc:4241)
     bool legacy = false;             // no handoff table: segment rows read from the payload (vp8_decoder.cc:337-369)
     bool zlib0 = false;              // magic CE B6 (zeta) instead of CF 84 (tau): the JPEG is handed out as a zlib stream
+    bool generic = false;            // the generic container of -permissive: the file is j.prefix, nothing is coded (nseg 0)
     uint32_t eee[7] = {0};
     std::vector<std::vector<uint8_t>> streams;   // demuxed per-segment bool-coder streams
     // read_lep(..., lazy = true): the mux packets of every stream as (pointer into the caller's file, length) instead of a

@@ -16,6 +16,9 @@
 // -embedding=N: every input is a JPEG whose SOI sits at byte N of the file, whatever its first two bytes (check_file,
 // jpgcoder.cc:2192); the N bytes in front of it are kept in the .lep and come back in front of the JPEG on restore.
 // -d: the .lep keeps only the header segments the coefficients are coded with (rebuild_header_jpg, jpgcoder.cc:4848).
+// -permissive: every input is compressed, whatever its first bytes and however short (jpgcoder.cc:1472, 1603), and verified
+// even with -skipverify; a file the coder cannot take -- or whose .lep would not restore it -- is stored whole in the
+// reference's generic container ('Y'), which restores it byte for byte.  Only an empty input still fails (42).
 // A .lep input may be a stream of concatenated .lep files (`cat a.lep b.lep | lepton-b200 -`, the reference's -lepcat files;
 // process_file, jpgcoder.cc:1867-1898): it is restored to the members' JPEGs one after the other, in single-file, stdin and
 // batch mode alike.  Writing -lepcat and -brotliheader files stays refused: both need brotli output identical to the
@@ -57,7 +60,7 @@ static std::string base_name(const std::string& path) {
 static bool is_lep_magic(const std::vector<uint8_t>& d) { return (d[0] == 0xCF && d[1] == 0x84) || (d[0] == 0xCE && d[1] == 0xB6); }
 
 static int run_batch(const std::vector<std::string>& files, const std::string& outdir, const std::vector<int>& devices, int allow_progressive, int min_threads, int max_threads, int even_split, int verify, int zlib0,
-                     long long embedding, int discard_meta) {
+                     long long embedding, int discard_meta, int permissive) {
     struct Item { std::string name; std::vector<uint8_t> data; bool is_jpeg = false, zeta = false; int status = 0; };
     std::vector<Item> items(files.size());
     int first_err = 0;
@@ -69,11 +72,11 @@ static int run_batch(const std::vector<std::string>& files, const std::string& o
         else {
             if (!read_all(f, it.data)) it.status = 33;
             fclose(f);
-            if (!it.status && it.data.size() < 2) it.status = 3;                                     // SHORT_READ
+            if (!it.status && it.data.size() < 2 && !permissive) it.status = 3;                      // SHORT_READ
         }
         if (!it.status) {
-            it.is_jpeg = embedding >= 0 || (it.data[0] == 0xFF && it.data[1] == 0xD8);
-            it.zeta = it.data[0] == 0xCE && it.data[1] == 0xB6;
+            it.is_jpeg = permissive || embedding >= 0 || (it.data[0] == 0xFF && it.data[1] == 0xD8);
+            it.zeta = !it.is_jpeg && it.data[0] == 0xCE && it.data[1] == 0xB6;
             if (!it.is_jpeg && !is_lep_magic(it.data)) it.status = 42;                              // UNSUPPORTED_JPEG
         }
     }
@@ -93,6 +96,7 @@ static int run_batch(const std::vector<std::string>& files, const std::string& o
         lepb200_codec_set_zlib0(c, zlib0);
         lepb200_codec_set_embedding(c, embedding);
         lepb200_codec_set_discard_meta(c, discard_meta);
+        lepb200_codec_set_permissive(c, permissive);
         codecs.push_back(c);
     }
     for (int dir = 0; dir < 2; ++dir) {                      // 0: JPEG -> .lep, 1: .lep -> JPEG
@@ -140,6 +144,7 @@ int main(int argc, char** argv) {
     int zlib0 = 0;               // -zlib0: restored JPEGs are written as zlib streams
     long long embedding = -1;    // -embedding=N: inputs are JPEGs at byte N of a larger file
     int discard_meta = 0;        // -d: metadata segments are left out of the .lep
+    int permissive = 0;          // -permissive: files the coder cannot take go into the generic container
     for (int i = 1; i < argc; ++i) {
         const char* a = argv[i];
         if (a[0] == '-' && a[1] != 0) {
@@ -159,6 +164,7 @@ int main(int argc, char** argv) {
             if (!strcmp(a, "-zlib0")) { zlib0 = 1; continue; }
             if (!strncmp(a, "-embedding=", 11)) { embedding = std::max(0ll, atoll(a + 11)); continue; }
             if (!strcmp(a, "-d")) { discard_meta = 1; continue; }
+            if (!strcmp(a, "-permissive")) { permissive = 1; continue; }
             if (!strcmp(a, "-allowprogressive") || !strcmp(a, "-forceprogressive")) { allow_progressive = 1; continue; }
             if (!strcmp(a, "-socket") || !strncmp(a, "-socket=", 8) || !strncmp(a, "-listen", 7) || !strcmp(a, "-fork") ||
                 !strcmp(a, "-benchmark") || !strcmp(a, "-lepcat") || !strncmp(a, "-startbyte", 10) || !strncmp(a, "-trunc=", 7) ||
@@ -176,14 +182,14 @@ int main(int argc, char** argv) {
         return 1;
     }
     if (devices.empty()) devices.push_back(device);
-    if (!outdir.empty()) return run_batch(files, outdir, devices, allow_progressive, min_threads, max_threads, even_split, verify, zlib0, embedding, discard_meta);
+    if (!outdir.empty()) return run_batch(files, outdir, devices, allow_progressive, min_threads, max_threads, even_split, verify, zlib0, embedding, discard_meta, permissive);
     std::vector<uint8_t> in;
     FILE* fi = files[0] == "-" ? stdin : fopen(files[0].c_str(), "rb");
     if (!fi) { fprintf(stderr, "lepton-b200: cannot open %s\n", files[0].c_str()); return 9; }   // FILE_NOT_FOUND
     if (!read_all(fi, in)) return 33;                                                            // OS_ERROR
     if (fi != stdin) fclose(fi);
-    if (in.size() < 2) return 3;                                                                 // SHORT_READ
-    const bool is_jpeg = embedding >= 0 || (in[0] == 0xFF && in[1] == 0xD8), is_lep = !is_jpeg && is_lep_magic(in);
+    if (in.size() < 2 && !permissive) return 3;                                                  // SHORT_READ
+    const bool is_jpeg = permissive || embedding >= 0 || (in[0] == 0xFF && in[1] == 0xD8), is_lep = !is_jpeg && is_lep_magic(in);
     const bool zlib_out = is_lep && (zlib0 || (in[0] == 0xCE && in[1] == 0xB6));
     if (!is_jpeg && !is_lep) { fprintf(stderr, "lepton-b200: input is neither JPEG nor Lepton\n"); return 42; }
     std::string outname;
@@ -205,6 +211,7 @@ int main(int argc, char** argv) {
     lepb200_codec_set_zlib0(codec, zlib0);
     lepb200_codec_set_embedding(codec, embedding);
     lepb200_codec_set_discard_meta(codec, discard_meta);
+    lepb200_codec_set_permissive(codec, permissive);
     lepb200_buffer ib = {in.data(), in.size()};
     lepb200_result res = {nullptr, 0, 0};
     rc = is_jpeg ? lepb200_compress_jpegs(codec, &ib, 1, &res) : lepb200_decompress_leps(codec, &ib, 1, &res);
