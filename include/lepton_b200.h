@@ -285,8 +285,8 @@ void lepb200_codec_set_even_split(lepb200_codec* codec, int on);
 /* -zlib0 (jpgcoder.cc:2089, check_file :2200-2220, src/io/Zlib0.cc): 1 = lepb200_decompress_leps hands every restored JPEG out
  * as a zlib stream: 78 01, stored deflate blocks of 65535 bytes (the last one BFINAL and never empty), the big-endian Adler-32
  * of the JPEG -- 2 + n + 5 ceil(n / 65535) + 4 bytes for an n-byte JPEG.  Files whose magic is CE B6 (zeta) instead of CF 84
- * are always handed out so, whatever this setting.  The Adler-32 of a scan the device re-encodes is taken by the encode kernel
- * (environment LEPB200_ZLIB0_HOST_ADLER=1: by the host, over every byte).  Statuses do not change; lepb200_compress_jpegs
+ * are always handed out so, whatever this setting.  The Adler-32 of a scan the device re-encodes is taken by the encode kernel,
+ * that of a scan the host re-encodes by the host.  Statuses do not change; lepb200_compress_jpegs
  * ignores the setting, as the reference does.  0 (default): plain JPEG bytes. */
 void lepb200_codec_set_zlib0(lepb200_codec* codec, int on);
 /* -embedding=N (jpgcoder.cc:1135-1137, read_jpeg :2275-2282): offset >= 0 makes lepb200_compress_jpegs take every input as a

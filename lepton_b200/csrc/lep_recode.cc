@@ -504,7 +504,7 @@ void zlib0_join(const std::vector<std::pair<const uint8_t*, size_t>>& parts, con
 }
 
 bool assemble_baseline(const LepFile& lf, const GpuRecodeSetup& gs, const uint8_t* scan, std::vector<uint8_t>& out, std::string& err,
-                       JpegOut mode, uint32_t scan_adler, uint32_t* member_adler) {
+                       bool zlib0, uint32_t scan_adler, uint32_t* member_adler) {
     const Jpeg& j = lf.j;
     const std::vector<uint8_t>& h = j.hdr;
     static const uint8_t soi[2] = {0xFF, 0xD8};
@@ -521,51 +521,37 @@ bool assemble_baseline(const LepFile& lf, const GpuRecodeSetup& gs, const uint8_
     size_t total = 0;
     for (const auto& pc : pieces) total += pc.second;
     if (total != lf.jpeg_size) { err = "re-created JPEG has the wrong size"; out.clear(); return false; }
-    if (mode == JpegOut::plain || member_adler) {
-        out.clear();
-        out.reserve((size_t)lf.jpeg_size + 16);
-        for (const auto& pc : pieces) out.insert(out.end(), pc.first, pc.first + pc.second);
-        if (!member_adler) return true;
-        if (mode == JpegOut::zlib0_host_adler) { *member_adler = (uint32_t)adler32(1, out.data(), (uInt)out.size()); return true; }
-        // the device's sum of the scan between the host's sums of the bytes in front of it and behind it
+    // the device took the scan's sum; the host sums the few header and trailer bytes and combines the three
+    auto adler = [&]() {
         uLong head = 1, tail = 1;
         size_t ntail = 0;
         for (int k = 0; k < 3; ++k) head = adler32(head, pieces[k].first, (uInt)pieces[k].second);
         for (int k = 4; k < 7; ++k) { tail = adler32(tail, pieces[k].first, (uInt)pieces[k].second); ntail += pieces[k].second; }
-        *member_adler = (uint32_t)adler32_combine(adler32_combine(head, scan_adler, (z_off_t)gs.scan_bytes), tail, (z_off_t)ntail);
+        return (uint32_t)adler32_combine(adler32_combine(head, scan_adler, (z_off_t)gs.scan_bytes), tail, (z_off_t)ntail);
+    };
+    if (!zlib0 || member_adler) {
+        out.clear();
+        out.reserve((size_t)lf.jpeg_size + 16);
+        for (const auto& pc : pieces) out.insert(out.end(), pc.first, pc.first + pc.second);
+        if (member_adler) *member_adler = adler();
         return true;
     }
-    const bool host_sum = mode == JpegOut::zlib0_host_adler;
-    Zlib0Writer w(out, total, host_sum);
-    if (host_sum) {
-        for (const auto& pc : pieces) w.put(pc.first, pc.second);
-        w.finish((uint32_t)w.adler);
-        return true;
-    }
-    // the device took the scan's sum; the host sums the few header and trailer bytes and combines the three
-    uLong head = 1, tail = 1;
-    size_t ntail = 0;
-    for (int k = 0; k < 7; ++k) {
-        w.put(pieces[k].first, pieces[k].second);
-        if (k < 3) head = adler32(head, pieces[k].first, (uInt)pieces[k].second);
-        if (k > 3) { tail = adler32(tail, pieces[k].first, (uInt)pieces[k].second); ntail += pieces[k].second; }
-    }
-    uLong a = adler32_combine(head, scan_adler, (z_off_t)gs.scan_bytes);
-    a = adler32_combine(a, tail, (z_off_t)ntail);
-    w.finish((uint32_t)a);
+    Zlib0Writer w(out, total, false);
+    for (const auto& pc : pieces) w.put(pc.first, pc.second);
+    w.finish(adler());
     return true;
 }
 
-bool recode_baseline(const LepFile& lf, const int16_t* const planes[4], std::vector<uint8_t>& out, std::string& err, JpegOut mode,
+bool recode_baseline(const LepFile& lf, const int16_t* const planes[4], std::vector<uint8_t>& out, std::string& err, bool zlib0,
                      uint32_t* member_adler) {
-    if (mode != JpegOut::plain && member_adler) {
-        if (!recode_baseline(lf, planes, out, err, JpegOut::plain)) return false;
+    if (zlib0 && member_adler) {
+        if (!recode_baseline(lf, planes, out, err)) return false;
         *member_adler = (uint32_t)adler32(1, out.data(), (uInt)out.size());
         return true;
     }
-    if (mode != JpegOut::plain) {
+    if (zlib0) {
         thread_local std::vector<uint8_t> jpeg;
-        if (!recode_baseline(lf, planes, jpeg, err, JpegOut::plain)) { out.clear(); return false; }
+        if (!recode_baseline(lf, planes, jpeg, err)) { out.clear(); return false; }
         zlib0_frame(jpeg.data(), jpeg.size(), out);
         return true;
     }

@@ -73,17 +73,15 @@ def test_dense_batch_decode_matches_reference_planes(monkeypatch, mode, lanes):
     dict(gpu_huffman=True),
     dict(gpu_huffman=False),
     dict(gpu_huffman=True, env={"LEPB200_HUFF_PAR": "0"}),
-    dict(gpu_huffman=True, env={"LEPB200_DEVICE_MUX": "0"}),
-    dict(gpu_huffman=True, env={"LEPB200_DEVICE_MUX": "1"}),
     dict(gpu_huffman=True, env={"LEPB200_RC_MODE": "0"}),
-    dict(gpu_huffman=False, env={"LEPB200_RC_MODE": "0", "LEPB200_DEVICE_MUX": "0"}),
+    dict(gpu_huffman=False, env={"LEPB200_RC_MODE": "0"}),
     # 256-bit sub-sequences: the 16-bit codes of some files do not resynchronise within the 62 iterations, so the serial
     # kernel redoes them on the device
     dict(gpu_huffman=True, env={"LEPB200_HUFF_SUBSEQ_BITS": "256", "LEPB200_TRACE": "1"}, serial_redo=True),
 ])
 def test_dense_files_compress_to_the_reference_lep_and_back(monkeypatch, capfd, cfg):
-    """File API (resident upload after the GPU Huffman decoder, or host planes; device or host container assembly;
-    both range-coder forms): the reference CLI's .lep byte for byte, and decompress restores every input."""
+    """File API (resident upload after the GPU Huffman decoder, or host planes; both range-coder forms): the reference
+    CLI's .lep byte for byte, and decompress restores every input."""
     from lepton_b200 import LeptonB200FileCodec
     for k, v in cfg.get("env", {}).items():
         monkeypatch.setenv(k, v)

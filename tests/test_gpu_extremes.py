@@ -91,8 +91,6 @@ def test_extreme_batch_decode_matches_reference_planes(monkeypatch, mode, lanes)
     dict(gpu_huffman=False),
     dict(gpu_huffman=True, env={"LEPB200_HUFF_PAR": "0"}),
     dict(gpu_huffman=True, env={"LEPB200_HUFF_PAR": "1", "LEPB200_HUFF_SUBSEQ_BITS": "512"}),
-    dict(gpu_huffman=True, env={"LEPB200_DEVICE_MUX": "0"}),
-    dict(gpu_huffman=True, env={"LEPB200_DEVICE_MUX": "1"}),
     # 256-bit sub-sequences: the 16-bit codes of some files do not resynchronise within the 62 iterations, so the serial
     # kernel redoes them on the device
     dict(gpu_huffman=True, env={"LEPB200_HUFF_SUBSEQ_BITS": "256", "LEPB200_TRACE": "1"}, serial_redo=True),

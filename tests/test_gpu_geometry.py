@@ -27,14 +27,12 @@ def md5(b):
     dict(gpu_huffman=False),
     dict(gpu_huffman=True, env={"LEPB200_HUFF_PAR": "0"}),
     dict(gpu_huffman=True, env={"LEPB200_HUFF_PAR": "1", "LEPB200_HUFF_SUBSEQ_BITS": "512"}),
-    dict(gpu_huffman=True, env={"LEPB200_DEVICE_MUX": "0"}),
-    dict(gpu_huffman=True, env={"LEPB200_DEVICE_MUX": "1"}),
-    dict(gpu_huffman=False, env={"LEPB200_RC_MODE": "0", "LEPB200_DEVICE_MUX": "0"}),
+    dict(gpu_huffman=False, env={"LEPB200_RC_MODE": "0"}),
 ])
 def test_geometry_files_compress_to_the_reference_lep_and_back(monkeypatch, cfg):
-    """File API over the whole corpus in one call (GPU or host Huffman decode, device or host container assembly, both
-    range-coder forms): the reference CLI's .lep byte for byte, or its exit status; decompress restores every input,
-    through the device Huffman encoder where it takes the file and the host re-encoder where it does not."""
+    """File API over the whole corpus in one call (GPU or host Huffman decode, both range-coder forms): the reference
+    CLI's .lep byte for byte, or its exit status; decompress restores every input, through the device Huffman encoder
+    where it takes the file and the host re-encoder where it does not."""
     from lepton_b200 import LeptonB200FileCodec
     for k, v in cfg.get("env", {}).items():
         monkeypatch.setenv(k, v)

@@ -166,13 +166,10 @@ def test_mixed_batch_many_images(codec):
         assert [x.data for x in g] == [r[1] for r in ref]
 
 
-@pytest.mark.parametrize("device_mux", ["1", "0"])
-def test_file_level_compress_matches_reference_lep_bytes(device_mux, monkeypatch):
-    """JPEG bytes -> .lep bytes through the file-level C ABI (host front end + CUDA coder + container) must equal
-    the file the unmodified reference CLI wrote for the same JPEG -- with the container assembled on the device
-    (lep_gather_kernel, the default) and by the host MuxWriter (LEPB200_DEVICE_MUX=0)."""
+def test_file_level_compress_matches_reference_lep_bytes():
+    """JPEG bytes -> .lep bytes through the file-level C ABI (host front end + CUDA coder + container assembled on the
+    device by lep_gather_kernel) must equal the file the unmodified reference CLI wrote for the same JPEG."""
     import os
-    monkeypatch.setenv("LEPB200_DEVICE_MUX", device_mux)
     from helpers import GOLDEN
     from lepton_b200 import LeptonB200FileCodec
     names = ["android.jpg", "androidcrop.jpg", "androidcropoptions.jpg", "androidtrail.jpg", "colorswap.jpg",

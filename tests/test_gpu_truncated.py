@@ -46,8 +46,6 @@ def photos():
 @pytest.mark.parametrize("cfg", [
     dict(gpu_huffman=True),
     dict(gpu_huffman=False),
-    dict(gpu_huffman=True, env={"LEPB200_DEVICE_MUX": "0"}),
-    dict(gpu_huffman=True, env={"LEPB200_DEVICE_MUX": "1"}),
     dict(gpu_huffman=True, env={"LEPB200_RC_MODE": "0"}),
 ])
 def test_every_cut_compresses_to_the_reference_lep_and_back(monkeypatch, cfg):

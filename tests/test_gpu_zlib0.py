@@ -61,15 +61,13 @@ def check_against_reference(rel, plain, got, ref):
         assert rel.startswith("truncated/") and "_t" in rel, rel
 
 
-@pytest.mark.parametrize("gpu_huffman,parts,host_adler", [(True, "1", "0"), (True, "4", "0"), (True, "1", "1"), (True, "4", "1"),
-                                                          (False, "4", "0")])
-def test_file_api_matches_reference(monkeypatch, gpu_huffman, parts, host_adler):
+@pytest.mark.parametrize("gpu_huffman,parts", [(True, "1"), (True, "4"), (False, "4")])
+def test_file_api_matches_reference(monkeypatch, gpu_huffman, parts):
     """Every committed .lep restored with zlib0=True, and its zeta copy restored with and without it, gives the reference's
     -zlib0 bytes, in one batch of 388 files (large enough for the device re-encode to run in parts); tau files of the same
     batch stay plain JPEGs.  Statuses are those of the plain restore."""
     from lepton_b200 import LeptonB200FileCodec
     monkeypatch.setenv("LEPB200_HENC_PARTS", parts)
-    monkeypatch.setenv("LEPB200_ZLIB0_HOST_ADLER", host_adler)
     leps = [read_golden(r) for r in LEPS]
     zetas = [zeta(l) for l in leps]
     fp = LeptonB200FileCodec(0, host_threads=8, gpu_huffman=gpu_huffman)
@@ -97,12 +95,10 @@ def test_file_api_matches_reference(monkeypatch, gpu_huffman, parts, host_adler)
         assert z_recoded == 0
 
 
-@pytest.mark.parametrize("host_adler", ["0", "1"])
-def test_length_sweep_through_the_library(monkeypatch, host_adler):
+def test_length_sweep_through_the_library():
     """The sweep's JPEGs (one block; one byte short of, at and past one and two blocks; three full blocks) compress to the
     reference's .lep and come back as the reference's -zlib0 bytes, on the device re-encode path."""
     from lepton_b200 import LeptonB200FileCodec
-    monkeypatch.setenv("LEPB200_ZLIB0_HOST_ADLER", host_adler)
     jpegs = [sweep_jpeg(r["total"]) for r in ZLIB0["sweep"]]
     fz = LeptonB200FileCodec(0, host_threads=4, zlib0=True)
     try:

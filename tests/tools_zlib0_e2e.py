@@ -1,9 +1,8 @@
 """Diagnostic (not a test): what zlib0 output costs when restoring .lep files through the file API.
 
 Config 2's corpus (1080p 4:2:0 q85, 32 distinct images replicated to N files) is compressed once, then `decompress` is timed
-in three settings on one codec, alternated round by round: zlib0 off; zlib0 on (the Adler-32 of device-encoded scans from
-the encode kernel); zlib0 on with LEPB200_ZLIB0_HOST_ADLER=1 (the host sums every byte).  Every setting's output is
-checked against the plain restore.  Prints one JSON line with the card, its power limit and the times.
+in two settings on one codec, alternated round by round: zlib0 off; zlib0 on (the Adler-32 of device-encoded scans from
+the encode kernel).  The zlib0 output is checked against the plain restore.  Prints one JSON line with the card, its power limit and the times.
 
     python tests/tools_zlib0_e2e.py [files] [rounds]
 """
@@ -30,13 +29,11 @@ r = fc.compress(jpegs)
 assert all(st == 0 for st, _ in r)
 handle = LeptonB200FileCodec.prepare([b for _, b in r])
 
-SETTINGS = {"plain": (0, "0"), "zlib0_kernel_adler": (1, "0"), "zlib0_host_adler": (1, "1")}
+SETTINGS = {"plain": 0, "zlib0_kernel_adler": 1}
 
 
 def use(name):
-    z, host = SETTINGS[name]
-    fc._L.lepb200_codec_set_zlib0(fc._c, z)
-    os.environ["LEPB200_ZLIB0_HOST_ADLER"] = host
+    fc._L.lepb200_codec_set_zlib0(fc._c, SETTINGS[name])
 
 
 # outputs first: every setting restores every file, and the zlib streams hold the plain JPEGs
@@ -44,12 +41,11 @@ use("plain")
 plain = fc.decompress(handle)
 assert all(st == 0 and out == j for (st, out), j in zip(plain, jpegs))
 gpu_recoded = fc.last_gpu_recoded
-for name in ("zlib0_kernel_adler", "zlib0_host_adler"):
-    use(name)
-    got = fc.decompress(handle)
-    for k in range(0, n, 97):
-        assert got[k][0] == 0 and zlib.decompress(got[k][1]) == plain[k][1], (name, k)
-    assert fc.last_gpu_recoded == gpu_recoded
+use("zlib0_kernel_adler")
+got = fc.decompress(handle)
+for k in range(0, n, 97):
+    assert got[k][0] == 0 and zlib.decompress(got[k][1]) == plain[k][1], k
+assert fc.last_gpu_recoded == gpu_recoded
 times = {k: [] for k in SETTINGS}
 for _ in range(rounds):
     for name in SETTINGS:
