@@ -67,7 +67,10 @@ _EXPORTS = [
     "lepb200_codec_set_embedding", "lepb200_codec_set_discard_meta", "lepb200_host_jpeg_open_embedded",
     "lepb200_host_lep_members", "lepb200_host_lep_open_member", "lepb200_encode_upload_tokens", "lepb200_encode_token_canaries", "lepb200_last_huffman_redone",
     "lepb200_codec_set_permissive", "lepb200_host_generic_lep", "lepb200_host_lep_generic",
+    "lepb200_decode_upload_coded", "lepb200_decode_upload_gather_coded", "lepb200_host_lep_coder",
 ]
+
+CODER_BOOL, CODER_ANS = 0, 1          # LEPB200_CODER_*: bool coder (container versions 1, 2, 4), rANS coder (version 3)
 
 
 def lib():
@@ -101,6 +104,8 @@ def lib():
     L.lepb200_encode_fetch.argtypes = [vp, sp]
     L.lepb200_decode_images.argtypes = [vp, ip, ctypes.c_int, sp, ctypes.POINTER(ctypes.c_int32)]
     L.lepb200_decode_upload.argtypes = [vp, ip, ctypes.c_int, sp]
+    L.lepb200_decode_upload_coded.argtypes = [vp, ip, ctypes.c_int, sp, ctypes.POINTER(ctypes.c_uint8)]
+    L.lepb200_decode_upload_coded.restype = ctypes.c_int
     L.lepb200_decode_launch.argtypes = [vp]
     L.lepb200_decode_fetch.argtypes = [vp, ip, ctypes.c_int, ctypes.POINTER(ctypes.c_int32)]
     for f in ("lepb200_encode_images", "lepb200_encode_upload", "lepb200_encode_launch", "lepb200_encode_fetch",
@@ -235,8 +240,9 @@ class LeptonB200Codec:
         self.encode_launch()
         return self.encode_fetch(copy=copy)
 
-    def decode_upload(self, images, streams):
-        """streams: per image, a list of per-segment byte strings"""
+    def decode_upload(self, images, streams, coders=None):
+        """streams: per image, a list of per-segment byte strings.  coders: per image, the entropy coder of its streams
+        (CODER_BOOL, or CODER_ANS for the rANS streams of container version 3); None = all CODER_BOOL."""
         n = sum(im.nseg for im in images)
         arr = (_Stream * n)()
         keep, k = [], 0
@@ -251,7 +257,13 @@ class LeptonB200Codec:
                 k += 1
         self._dec_imgs, self._dec_keep = images, keep
         self._dec_c = self._c_images(images)
-        self._check(self._L.lepb200_decode_upload(self._ctx, self._dec_c, len(images), arr), "decode_upload")
+        if coders is None:
+            self._check(self._L.lepb200_decode_upload(self._ctx, self._dec_c, len(images), arr), "decode_upload")
+        else:
+            if len(coders) != len(images):
+                raise LeptonB200Error("one coder per image")
+            cod = (ctypes.c_uint8 * len(images))(*[int(c) for c in coders])
+            self._check(self._L.lepb200_decode_upload_coded(self._ctx, self._dec_c, len(images), arr, cod), "decode_upload")
 
     def decode_launch(self):
         self._check(self._L.lepb200_decode_launch(self._ctx), "decode_launch")
@@ -279,9 +291,10 @@ class LeptonB200Codec:
         self._check(self._L.lepb200_decode_fetch(self._ctx, c, len(self._dec_imgs), st), "decode_fetch")
         return list(st)
 
-    def decode_images(self, images, streams):
-        """Decodes into ``images[i].planes`` (pre-allocated).  Returns per-segment status codes."""
-        self.decode_upload(images, streams)
+    def decode_images(self, images, streams, coders=None):
+        """Decodes into ``images[i].planes`` (pre-allocated).  Returns per-segment status codes.  coders: per image,
+        CODER_BOOL or CODER_ANS (the rANS streams of container version 3, HostLep.coder()); None = all CODER_BOOL."""
+        self.decode_upload(images, streams, coders)
         self.decode_launch()
         return self.decode_fetch()
 
@@ -417,6 +430,8 @@ def _bind_file_api(L):
     L.lepb200_codec_set_zlib0.restype = None
     L.lepb200_host_lep_zlib0.argtypes = [vp]
     L.lepb200_host_lep_zlib0.restype = ctypes.c_int
+    L.lepb200_host_lep_coder.argtypes = [vp]
+    L.lepb200_host_lep_coder.restype = ctypes.c_int
     L.lepb200_host_zlib0_frame.argtypes = [ctypes.c_char_p, ctypes.c_size_t, ctypes.c_void_p, ctypes.c_size_t]
     L.lepb200_host_zlib0_frame.restype = ctypes.c_size_t
     L.lepb200_host_jpeg_error.argtypes = [vp]
@@ -558,6 +573,10 @@ class HostLep:
     def zlib0(self) -> bool:
         """True for a container with the zeta magic (CE B6): its JPEG is restored as a zlib stream."""
         return bool(self._L.lepb200_host_lep_zlib0(self._h))
+
+    def coder(self) -> int:
+        """CODER_ANS for a container of version 3 (rANS-coded streams), else CODER_BOOL: its coder for decode_images."""
+        return int(self._L.lepb200_host_lep_coder(self._h))
 
     def restore_generic(self, zlib0: bool = False) -> bytes:
         """The bytes a generic container of -permissive restores to (zlib0=True: as a zlib stream of stored blocks)."""

@@ -124,6 +124,9 @@ struct lepb200_ctx {
     int dec_lanes = 4;                    // group kernel: lanes per thread-segment, 32 / dec_lanes segments per warp in lock step
     int dec_group_grid = 0;               // group kernel: CTAs of the current batch
     int dec_threads = 0;                  // group kernel: model slots of the current batch (0: the batch uses the warp kernel)
+    // decode batches with rANS-coded segments (lepb200_decode_upload_coded): they follow the bool-coded ones in the launch
+    // order (BatchPlan::order_ans) and are decoded by launches of their own, group kernel or warp kernel by their own count
+    int dec_threads_ans = 0, dec_group_grid_ans = 0, grid_ans = 0;
     bool stage_preuploaded = false;       // the caller pushed the staged scans itself (lepb200_huffman_stage_upload)
     bool canary = false;                  // batch of lepb200_encode_upload_tokens: stream and overflow arenas hold canary bytes
     size_t rc_ovf_used = 0;               // bytes of the overflow arena the last range coder run placed streams in
@@ -148,7 +151,8 @@ namespace {
 // lep_decode_g2_kernel<G>: launch shape (warps per CTA, thread-segments per warp) and resident CTAs per SM.  The groups'
 // front regions take G2Cfg<G>::HOT_BYTES of dynamic shared memory (75 KB at G = 4: 32 groups of 2 400 bytes), more than the default 48 KB limit.
 template <int G> cudaError_t group_kernel_allow_smem() {
-    return cudaFuncSetAttribute(lep_decode_g2_kernel<G>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)G2Cfg<G>::HOT_BYTES);
+    const cudaError_t e = cudaFuncSetAttribute(lep_decode_g2_kernel<G, G2Bool>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)G2Cfg<G>::HOT_BYTES);
+    return e != cudaSuccess ? e : cudaFuncSetAttribute(lep_decode_g2_kernel<G, G2Ans>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)G2Cfg<G>::HOT_BYTES);
 }
 template <int G> int group_ctas_per_sm() {
     int n = 0;
@@ -163,26 +167,65 @@ void group_launch_shape(int lanes, int& warps, int& per_warp, int& ctas_per_sm) 
     default: warps = G2Cfg<4>::WARPS; ctas_per_sm = group_ctas_per_sm<4>(); break;
     }
 }
-template <int G> void launch_group_kernel(int grid, cudaStream_t st, const ImageDesc* images, SegDesc* segs, int first, int count, const int* order,
+template <int G, class Coder = G2Bool> void launch_group_kernel(int grid, cudaStream_t st, const ImageDesc* images, SegDesc* segs, int first, int count, const int* order,
                                           int* counter, uint16_t* models, uint8_t* rows, size_t row_stride) {
-    lep_decode_g2_kernel<G><<<grid, G2Cfg<G>::THREADS, G2Cfg<G>::HOT_BYTES, st>>>(images, segs, first, count, order, counter, models, rows, row_stride);
+    lep_decode_g2_kernel<G, Coder><<<grid, G2Cfg<G>::THREADS, G2Cfg<G>::HOT_BYTES, st>>>(images, segs, first, count, order, counter, models, rows, row_stride);
 }
 
+// The decode launches of one coder's segments, order[first .. first + n): the group kernel in launches of at most `threads`
+// segments (threads > 0), else the warp kernel on a persistent grid of `wgrid` CTAs.
+template <class WarpReader, class GroupCoder> int decode_launch_part(lepb200_ctx* ctx, int first, int n, int threads, int ggrid, int wgrid) {
+    const ImageDesc* di = static_cast<const ImageDesc*>(ctx->d_images.p);
+    SegDesc* ds = static_cast<SegDesc*>(ctx->d_segs.p);
+    const int* dord = static_cast<const int*>(ctx->d_order.p);
+    int* dcnt = static_cast<int*>(ctx->d_counter.p);
+    uint16_t* dm = static_cast<uint16_t*>(ctx->d_models.p);
+    uint8_t* dr = static_cast<uint8_t*>(ctx->d_rows.p);
+    if (threads > 0) {
+        // group kernel (lep_decode_g2.cu): G lanes per segment, 32 / G segments per warp in lock step; the groups of a
+        // launch share a queue of at most dec_threads segments (one zero-filled model each), largest first
+        int warps = 0, per_warp = 0, gsm = 0;
+        group_launch_shape(ctx->dec_lanes, warps, per_warp, gsm);
+        const int per_cta = warps * per_warp;
+        for (int off = 0; off < n; off += threads) {
+            const int count = std::min(threads, n - off);
+            const int grid = std::max(1, std::min(ggrid, (count + per_cta - 1) / per_cta));
+            CK(cudaMemsetAsync(ctx->d_models.p, 0, (size_t)count * MODEL_BYTES, ctx->stream));       // identity prior = zero fill
+            CK(cudaMemsetAsync(ctx->d_counter.p, 0, sizeof(int), ctx->stream));
+            switch (ctx->dec_lanes) {
+            case 8: launch_group_kernel<8, GroupCoder>(grid, ctx->stream, di, ds, first + off, count, dord, dcnt, dm, dr, ctx->batch.row_stride); break;
+            case 32: launch_group_kernel<32, GroupCoder>(grid, ctx->stream, di, ds, first + off, count, dord, dcnt, dm, dr, ctx->batch.row_stride); break;
+            default: launch_group_kernel<4, GroupCoder>(grid, ctx->stream, di, ds, first + off, count, dord, dcnt, dm, dr, ctx->batch.row_stride); break;
+            }
+            CK(cudaGetLastError());
+            ctx->launches += 1;
+        }
+    } else {
+        if (first > 0) CK(cudaMemsetAsync(ctx->d_counter.p, 0, sizeof(int), ctx->stream));    // the batch's first queue: cleared before ev0
+        lep_decode_kernel<WarpReader><<<wgrid, DEC_WARPS_PER_CTA * 32, 0, ctx->stream>>>(di, ds, n, dord + first, dcnt, dm, dr, ctx->batch.row_stride);
+        CK(cudaGetLastError());
+        ctx->launches += 1;
+    }
+    return LEPB200_OK;
+}
 // Common part of encode/decode upload: job tables (lep_plan.cuh), launch shape, pools, upload of the tables.
-int build_batch(lepb200_ctx* ctx, const lepb200_image* images, int nimages, bool encode, const lepb200_stream* in) {
+int build_batch(lepb200_ctx* ctx, const lepb200_image* images, int nimages, bool encode, const lepb200_stream* in,
+                const uint8_t* coders = nullptr) {
     ctx->have_batch = false; ctx->launched = false; ctx->is_encode = encode; ctx->canary = false;
     BatchPlan& b = ctx->batch;
-    if (const char* e = plan_batch(b, images, nimages, encode, in)) { ctx->err = e; return LEPB200_ERR_INVALID; }
+    if (const char* e = plan_batch(b, images, nimages, encode, in, coders)) { ctx->err = e; return LEPB200_ERR_INVALID; }
     const int nseg = (int)b.segs.size();
+    const int nbool = encode ? nseg : b.order_ans;      // decode: the bool-coded segments, launched before the rANS-coded ones
 
     // persistent grid: as many CTAs as can be resident, but no more warps than segments
     int per_sm = 0;
     if (encode) CK(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, lep_encode_kernel, ENC_WARPS_PER_CTA * 32, 0));
-    else CK(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, lep_decode_kernel, DEC_WARPS_PER_CTA * 32, 0));
+    else CK(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, lep_decode_kernel<BoolReader>, DEC_WARPS_PER_CTA * 32, 0));
     if (encode && ctx->enc_cta_cap > 0) per_sm = std::min(per_sm, ctx->enc_cta_cap);
     const int wpc = encode ? ENC_WARPS_PER_CTA : DEC_WARPS_PER_CTA;
-    int grid = std::max(1, std::min(per_sm * ctx->sm_count, (nseg + wpc - 1) / wpc));
+    int grid = std::max(1, std::min(per_sm * ctx->sm_count, (nbool + wpc - 1) / wpc));
     ctx->grid = grid;
+    ctx->grid_ans = std::max(1, std::min(per_sm * ctx->sm_count, (nseg - nbool + wpc - 1) / wpc));
 
     CK(ctx->d_planes.reserve(b.plane_total));
     CK(ctx->d_streams.reserve(b.stream_total + 256));
@@ -190,21 +233,30 @@ int build_batch(lepb200_ctx* ctx, const lepb200_image* images, int nimages, bool
     CK(ctx->d_segs.reserve(sizeof(SegDesc) * nseg));
     CK(ctx->d_order.reserve(sizeof(int) * nseg));
     CK(ctx->d_counter.reserve(256));
-    ctx->dec_threads = 0;
-    const bool use_group = !encode && (ctx->dec_mode == 2 || (ctx->dec_mode == 0 && nseg >= ctx->dec_group_min));
-    if (use_group) {
-        // group kernel: one zero-filled model per segment of a launch, one row buffer per resident group
-        ctx->dec_threads = std::max(1, std::min(nseg, ctx->dec_threads_max));
-        int warps = 0, per_warp = 0, gsm = 0;
-        group_launch_shape(ctx->dec_lanes, warps, per_warp, gsm);
-        const int per_cta = warps * per_warp;
-        ctx->dec_group_grid = std::max(1, std::min(gsm * ctx->sm_count, (ctx->dec_threads + per_cta - 1) / per_cta));
-        CK(ctx->d_models.reserve((size_t)ctx->dec_threads * MODEL_BYTES));
-        CK(ctx->d_rows.reserve((size_t)ctx->dec_group_grid * per_cta * b.row_stride));
-    } else {
-        CK(ctx->d_models.reserve((size_t)grid * wpc * MODEL_BYTES));
-        CK(ctx->d_rows.reserve((size_t)grid * wpc * b.row_stride));
-    }
+    // decode kernel of each coder's segments: the group kernel when there are at least dec_group_min of them (one zero-filled
+    // model per segment of a launch, one row buffer per resident group), else the warp kernel (one model and row buffer per warp)
+    size_t model_bytes = 0, row_bytes = 0;
+    auto part = [&](int n, int wgrid, int& threads, int& ggrid) {
+        threads = 0;
+        if (n == 0) return;
+        const bool use_group = !encode && (ctx->dec_mode == 2 || (ctx->dec_mode == 0 && n >= ctx->dec_group_min));
+        if (use_group) {
+            threads = std::max(1, std::min(n, ctx->dec_threads_max));
+            int warps = 0, per_warp = 0, gsm = 0;
+            group_launch_shape(ctx->dec_lanes, warps, per_warp, gsm);
+            const int per_cta = warps * per_warp;
+            ggrid = std::max(1, std::min(gsm * ctx->sm_count, (threads + per_cta - 1) / per_cta));
+            model_bytes = std::max(model_bytes, (size_t)threads * MODEL_BYTES);
+            row_bytes = std::max(row_bytes, (size_t)ggrid * per_cta * b.row_stride);
+        } else {
+            model_bytes = std::max(model_bytes, (size_t)wgrid * wpc * MODEL_BYTES);
+            row_bytes = std::max(row_bytes, (size_t)wgrid * wpc * b.row_stride);
+        }
+    };
+    part(nbool, grid, ctx->dec_threads, ctx->dec_group_grid);
+    part(nseg - nbool, ctx->grid_ans, ctx->dec_threads_ans, ctx->dec_group_grid_ans);
+    CK(ctx->d_models.reserve(model_bytes));
+    CK(ctx->d_rows.reserve(row_bytes));
     for (auto& d : b.images)
         for (int c = 0; c < d.ncmp; ++c) d.plane[c] += (unsigned long long)(uintptr_t)ctx->d_planes.p;
     for (auto& sd : b.segs) sd.stream += (unsigned long long)(uintptr_t)ctx->d_streams.p;
@@ -1028,11 +1080,11 @@ int lepb200_huffman_encode_adler32(lepb200_ctx* ctx, int first, int last, uint32
 
 // ------------------------------------------------------------------------------------------------ decode
 static int decode_upload_impl(lepb200_ctx* ctx, const lepb200_image* images, int nimages, const lepb200_stream* in,
-                              const lepb200_buffer* spans, const uint32_t* span_first) {
+                              const lepb200_buffer* spans, const uint32_t* span_first, const uint8_t* coders) {
     if (!ctx || !in) return LEPB200_ERR_INVALID;
     CK(cudaSetDevice(ctx->device));
     ctx->d_tokens.release();              // the encoder's token arena (the largest buffer of that direction) is not needed on the way back
-    int r = build_batch(ctx, images, nimages, false, in);
+    int r = build_batch(ctx, images, nimages, false, in, coders);
     if (r) return r;
     const int nseg = (int)ctx->batch.segs.size();
     // planes start zeroed: blocks outside the coded range (truncated images) stay zero like the reference's calloc.
@@ -1082,56 +1134,39 @@ static int decode_upload_impl(lepb200_ctx* ctx, const lepb200_image* images, int
 }
 
 int lepb200_decode_upload(lepb200_ctx* ctx, const lepb200_image* images, int nimages, const lepb200_stream* in) {
-    return decode_upload_impl(ctx, images, nimages, in, nullptr, nullptr);
+    return decode_upload_impl(ctx, images, nimages, in, nullptr, nullptr, nullptr);
 }
 
 int lepb200_decode_upload_gather(lepb200_ctx* ctx, const lepb200_image* images, int nimages, const lepb200_stream* in,
                                  const lepb200_buffer* spans, const uint32_t* span_first) {
     if (!spans || !span_first) return LEPB200_ERR_INVALID;
-    return decode_upload_impl(ctx, images, nimages, in, spans, span_first);
+    return decode_upload_impl(ctx, images, nimages, in, spans, span_first, nullptr);
+}
+
+int lepb200_decode_upload_coded(lepb200_ctx* ctx, const lepb200_image* images, int nimages, const lepb200_stream* in,
+                                const uint8_t* coders) {
+    return decode_upload_impl(ctx, images, nimages, in, nullptr, nullptr, coders);
+}
+
+int lepb200_decode_upload_gather_coded(lepb200_ctx* ctx, const lepb200_image* images, int nimages, const lepb200_stream* in,
+                                       const lepb200_buffer* spans, const uint32_t* span_first, const uint8_t* coders) {
+    if (!spans || !span_first) return LEPB200_ERR_INVALID;
+    return decode_upload_impl(ctx, images, nimages, in, spans, span_first, coders);
 }
 
 int lepb200_decode_launch(lepb200_ctx* ctx) {
     if (!ctx || !ctx->have_batch || ctx->is_encode) { if (ctx) ctx->err = "decode_launch without decode_upload"; return LEPB200_ERR_INVALID; }
     CK(cudaSetDevice(ctx->device));
     const int nseg = (int)ctx->batch.segs.size();
+    const int nbool = ctx->batch.order_ans;
     CK(cudaMemsetAsync(ctx->d_counter.p, 0, sizeof(int), ctx->stream));
     CK(cudaEventRecord(ctx->ev0, ctx->stream));
-    if (ctx->dec_threads > 0) {
-        // group kernel (lep_decode_g2.cu): G lanes per segment, 32 / G segments per warp in lock step; the groups of a
-        // launch share a queue of at most dec_threads segments (one zero-filled model each), largest first
-        int warps = 0, per_warp = 0, gsm = 0;
-        group_launch_shape(ctx->dec_lanes, warps, per_warp, gsm);
-        const int per_cta = warps * per_warp;
-        for (int first = 0; first < nseg; first += ctx->dec_threads) {
-            const int count = std::min(ctx->dec_threads, nseg - first);
-            const int grid = std::max(1, std::min(ctx->dec_group_grid, (count + per_cta - 1) / per_cta));
-            CK(cudaMemsetAsync(ctx->d_models.p, 0, (size_t)count * MODEL_BYTES, ctx->stream));       // identity prior = zero fill
-            CK(cudaMemsetAsync(ctx->d_counter.p, 0, sizeof(int), ctx->stream));
-            const ImageDesc* di = static_cast<const ImageDesc*>(ctx->d_images.p);
-            SegDesc* ds = static_cast<SegDesc*>(ctx->d_segs.p);
-            const int* dord = static_cast<const int*>(ctx->d_order.p);
-            int* dcnt = static_cast<int*>(ctx->d_counter.p);
-            uint16_t* dm = static_cast<uint16_t*>(ctx->d_models.p);
-            uint8_t* dr = static_cast<uint8_t*>(ctx->d_rows.p);
-            switch (ctx->dec_lanes) {
-            case 8: launch_group_kernel<8>(grid, ctx->stream, di, ds, first, count, dord, dcnt, dm, dr, ctx->batch.row_stride); break;
-            case 32: launch_group_kernel<32>(grid, ctx->stream, di, ds, first, count, dord, dcnt, dm, dr, ctx->batch.row_stride); break;
-            default: launch_group_kernel<4>(grid, ctx->stream, di, ds, first, count, dord, dcnt, dm, dr, ctx->batch.row_stride); break;
-            }
-            CK(cudaGetLastError());
-            ctx->launches += 1;
-        }
-        ctx->launches -= 1;
-    } else {
-        lep_decode_kernel<<<ctx->grid, DEC_WARPS_PER_CTA * 32, 0, ctx->stream>>>(
-            static_cast<const ImageDesc*>(ctx->d_images.p), static_cast<SegDesc*>(ctx->d_segs.p), nseg, static_cast<const int*>(ctx->d_order.p),
-            static_cast<int*>(ctx->d_counter.p), static_cast<uint16_t*>(ctx->d_models.p), static_cast<uint8_t*>(ctx->d_rows.p), ctx->batch.row_stride);
-        CK(cudaGetLastError());
-    }
+    int r = nbool > 0 ? decode_launch_part<BoolReader, G2Bool>(ctx, 0, nbool, ctx->dec_threads, ctx->dec_group_grid, ctx->grid) : LEPB200_OK;
+    if (r == LEPB200_OK && nseg > nbool)
+        r = decode_launch_part<AnsReader, G2Ans>(ctx, nbool, nseg - nbool, ctx->dec_threads_ans, ctx->dec_group_grid_ans, ctx->grid_ans);
+    if (r) return r;
     CK(cudaEventRecord(ctx->ev1, ctx->stream));
     ctx->status_queued = false;
-    ctx->launches += 1;
     ctx->launched = true;
     return LEPB200_OK;
 }

@@ -170,7 +170,7 @@ struct ImageDesc {
     int32_t trunc_bcv[3];            // rows actually coded   (UncompressedComponents::get_max_coded_heights)
     int32_t trunc_bc[3];             // blocks actually coded (component_size_in_blocks)
     int32_t mult[3];                 // bcv / mcuv: component rows per MCU row (lepton_codec.hh:55-57)
-    int32_t pad_;
+    int32_t coder;                   // decode: entropy coder of the image's streams (CODER_BOOL, CODER_ANS); a launch takes one coder's segments
     unsigned long long plane[3];     // device address of the component's coefficient plane (AlignedBlock order)
     uint16_t q[3][64];               // quantisation table, raster order (model.hh:248-250)
     int32_t icos_x[3][64];           // model.hh:254
@@ -194,6 +194,11 @@ struct SegDesc {
     unsigned long long ovf;          // encode, parallel range coder: 1 + offset of the segment's stream in the overflow arena when
                                      // the stream does not fit `cap` (lep_digit_offsets_kernel), 0 when it stays where it is
 };
+
+// Entropy coders of a segment's stream: the VP8 bool coder of container versions 1, 2 and 4, or the two-state rANS coder of
+// version 3 (the reference's -ans, ans_bool_reader.hh).  Same grammar and model layout; the rANS coder has its own update of
+// the branch counts (branch_update_ans) and its own bits.
+enum : int32_t { CODER_BOOL = 0, CODER_ANS = 1 };
 
 enum : int32_t { ST_OK = 0, ST_ASSERT = 1, ST_COEF_RANGE = 6, ST_STREAM_INCONSISTENT = 7, ST_OUT_OVERFLOW = 100 };
 
@@ -228,6 +233,22 @@ __device__ __forceinline__ uint32_t branch_update(uint32_t w, uint32_t obs) {
             c0 += 1;
         }
     }
+    return (c0 - 1) | ((c1 - 1) << 8);
+}
+
+// The rANS coder's model (ANSBoolReader::get and ANSBoolWriter::put call Branch::adv_record_obs_and_update, branch.hh:60-77):
+// the observed count goes up, and from 255 it restarts at 129 while the other count is halved (rounded up); the probability
+// is the same quotient with its low bit set, so it is never 0 and the special state of the bool coder's model never arises.
+// Only a branch that was never updated (the zero word, counts (1, 1)) keeps its initial probability 128 (set_identity).
+__device__ __forceinline__ uint32_t branch_prob_ans(uint32_t w, const uint32_t* __restrict__ s_rcp) {
+    uint32_t lo = w & 0xff, hi = (w >> 8) & 0xff;
+    uint32_t c0 = lo + 1, s = lo + hi + 2;
+    return w == 0 ? 128u : __umulhi(c0 << 8, s_rcp[s]) | 1u;
+}
+__device__ __forceinline__ uint32_t branch_update_ans(uint32_t w, uint32_t obs) {
+    uint32_t c0 = (w & 0xff) + 1, c1 = ((w >> 8) & 0xff) + 1;
+    if (obs) { if (c1 == 255) { c1 = 129; c0 = (c0 + 1) >> 1; } else { c1 += 1; } }
+    else { if (c0 == 255) { c0 = 129; c1 = (c1 + 1) >> 1; } else { c0 += 1; } }
     return (c0 - 1) | ((c1 - 1) << 8);
 }
 

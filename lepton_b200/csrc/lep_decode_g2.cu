@@ -87,6 +87,8 @@ __device__ __forceinline__ uint32_t g2_model_word(uint32_t w, uint32_t bit) {
     const bool plain = (w & 0xffu) < 254u && (w >> 8) < 254u;       // no count about to saturate, not the special state
     return (plain ? w + (bit ? 0x100u : 1u) : branch_update(w, bit)) & 0xffffu;
 }
+// the branch word after the observation, in the model of the segment's coder
+__device__ __forceinline__ uint32_t g2_next_word(const G2Bool&, uint32_t w, uint32_t bit) { return g2_model_word(w, bit); }
 // one whole decision where nothing is pipelined (fixed-length count loops use the pieces directly)
 __device__ __forceinline__ uint32_t g2_get(G2Bool& r, uint16_t* model, const uint32_t* rcp, uint32_t addr, uint32_t w) {
     uint32_t split;
@@ -95,6 +97,58 @@ __device__ __forceinline__ uint32_t g2_get(G2Bool& r, uint16_t* model, const uin
     model[addr] = (uint16_t)g2_model_word(w, bit);                 // all lanes of the group store the same value
     return bit;
 }
+__device__ __forceinline__ void g2_reset(G2Bool& r) { r.value = 0; r.valid = 0; r.range = 255; r.next = 0; r.p = nullptr; r.end = nullptr; }
+
+// ANSBoolReader (ans_bool_reader.hh:75-108, rans64.hh:108-139) in the same three pieces.  The decision reads the low byte of
+// a state that was final two decisions ago, so the chain is only branch word -> probability -> compare; the state update
+// and its refill word are off it.  Which word the refill takes depends only on how many words were taken before, never on
+// their values: the next one is loaded right after the previous one is used.
+struct G2Ans {                            // identical in the G lanes of a group
+    unsigned long long x0, x1;            // state of the next decision, of the one after it
+    uint32_t next;                        // the next 32-bit word of the stream (little-endian), already loaded
+    const uint8_t* p;                     // address `next` was loaded from
+    const uint8_t* end;
+};
+__device__ __forceinline__ void g2_reset(G2Ans& r) { r.x0 = 0; r.x1 = 0; r.next = 0; r.p = nullptr; r.end = nullptr; }
+__device__ __forceinline__ uint32_t g2_ans_word(const uint8_t* p, const uint8_t* end) {
+    uint32_t w = 0;
+    const long long rem = end - p;
+    if (rem > 0) {
+        w = __ldg(reinterpret_cast<const uint32_t*>(p));
+        if (rem < 4) w &= 0xffffffffu >> (8 * (4 - (int)rem));         // the padding behind a stream is readable but not zero
+    }
+    return w;
+}
+// Rans64DecInit twice (words 0-1, then 2-3, low word first); word 4 is requested right away
+__device__ __forceinline__ void g2_init(G2Ans& r, const uint8_t* p, uint32_t len) {
+    r.p = p; r.end = p + len;
+    r.x0 = (unsigned long long)g2_ans_word(p, r.end) | (unsigned long long)g2_ans_word(p + 4, r.end) << 32;
+    r.x1 = (unsigned long long)g2_ans_word(p + 8, r.end) | (unsigned long long)g2_ans_word(p + 12, r.end) << 32;
+    r.p = p + 16;
+    r.next = g2_ans_word(r.p, r.end);
+}
+// Rans64DecGet at scale 8 against the probability of the rANS coder's model; `prob` is kept for the update
+__device__ __forceinline__ uint32_t g2_bit(G2Ans& r, const uint32_t* rcp, uint32_t w, uint32_t& prob) {
+    prob = branch_prob_ans(w, rcp);
+    return ((uint32_t)r.x0 & 255u) >= prob;
+}
+// Rans64DecAdvance (at most one word), then the states take turns
+__device__ __forceinline__ void g2_update(G2Ans& r, uint32_t prob, uint32_t bit) {
+    const unsigned long long x = r.x0;
+    const uint32_t cf = (uint32_t)x & 255u;
+    const uint32_t start = bit ? prob : 0u;
+    const uint32_t freq = (prob ^ (0u - bit)) + (bit | (bit << 8));  // bit ? 256 - prob : prob
+    unsigned long long nx = (unsigned long long)freq * (x >> 8) + cf - start;
+    if (nx < (1ull << 31)) {
+        nx = (nx << 32) | r.next;
+        r.p += 4;
+        r.next = g2_ans_word(r.p, r.end);
+    }
+    r.x0 = r.x1;
+    r.x1 = nx;
+}
+__device__ __forceinline__ uint32_t g2_next_word(const G2Ans&, uint32_t w, uint32_t bit) { return branch_update_ans(w, bit); }
+
 #ifdef LEPB200_EMU
 #define G2_EMU_BARRIER() __syncwarp()      // CPU warp emulator only: lanes run one after the other there, so the lanes of a group must
                                            // all have read a branch word before the first of them writes it back (fixed-length count loops;
@@ -205,7 +259,9 @@ __device__ __forceinline__ uint32_t g2_edge_info(int prior, int min_thr) {
     return (uint32_t)bsr | ((uint32_t)sctx << 4) | ((uint32_t)min_thr << 6) | ((uint32_t)min(ctx_abs >> min_thr, 255) << 9);
 }
 
-template <int G>
+// Coder: G2Bool (container versions 1, 2, 4) or G2Ans (version 3).  The groups of a warp run in lock step, so every segment
+// of a launch uses the launch's coder.
+template <int G, class Coder = G2Bool>
 __global__ void __launch_bounds__(G2Cfg<G>::THREADS)
 lep_decode_g2_kernel(const ImageDesc* __restrict__ images, SegDesc* __restrict__ segs, int first, int count, const int* __restrict__ order,
                      int* __restrict__ work_counter, uint16_t* __restrict__ model_pool, uint8_t* __restrict__ row_pool, size_t row_pool_stride) {
@@ -248,8 +304,8 @@ lep_decode_g2_kernel(const ImageDesc* __restrict__ images, SegDesc* __restrict__
     uint32_t mwidth = 1;                  // models in the interleave block of `model`
     int seg_min_y = 0, seg_max_y = 0;
     bool seg_last = false;
-    G2Bool br;
-    br.value = 0; br.valid = 0; br.range = 255; br.next = 0; br.p = nullptr; br.end = nullptr;
+    Coder br;
+    g2_reset(br);
     unsigned long long ndec = 0;
     uint32_t top_mask = 7u, index = 0;
     int bw0 = 0, bw1 = 0, bw2 = 0, nzs0 = 0, nzs1 = 0;
@@ -411,7 +467,7 @@ lep_decode_g2_kernel(const ImageDesc* __restrict__ images, SegDesc* __restrict__
                 if (alive && idx == 4) r0 = g2_units4(model, mwidth, cnt_rear + nz7_row(0) + (p1 << 3));
                 if (idx >= 4) G2_EMU_BARRIER();
                 if (alive) {
-                    const uint16_t neww = (uint16_t)g2_model_word(mw, bit);
+                    const uint16_t neww = (uint16_t)g2_next_word(br, mw, bit);
                     if (idx >= 3) hot[cnt_top + (nz7_row(idx) - nz7_row(3)) + prefix] = neww;
                     else g2_gword(model, mwidth, cnt_rear + nz7_row(idx) + prefix) = neww;
                     g2_update(br, split, bit);
@@ -452,7 +508,7 @@ lep_decode_g2_kernel(const ImageDesc* __restrict__ images, SegDesc* __restrict__
                     const bool nbusy = bit ? b1 : b0;
                     uint32_t mwn = nbusy ? *g2_word(hot, model, mwidth, naddr) : 0u;
                     // ---- in the shadow of that load: write-back, window, grammar state, decoded value
-                    const uint32_t neww = g2_model_word(mw, bit);
+                    const uint32_t neww = g2_next_word(br, mw, bit);
                     *g2_word(hot, model, mwidth, addr) = (uint16_t)neww;   // all lanes of the group store the same value
                     if (naddr == addr) mwn = neww;
                     g2_update(br, split, bit);
@@ -544,7 +600,7 @@ lep_decode_g2_kernel(const ImageDesc* __restrict__ images, SegDesc* __restrict__
                     uint32_t split = 0, bit = 0;
                     if (alive) {
                         bit = g2_bit(br, s_rcp, mw, split);
-                        g2_gword(model, mwidth, base + ((uint32_t)idx << 2) + prefix) = (uint16_t)g2_model_word(mw, bit);
+                        g2_gword(model, mwidth, base + ((uint32_t)idx << 2) + prefix) = (uint16_t)g2_next_word(br, mw, bit);
                         g2_update(br, split, bit);
                         prefix = (prefix << 1) | bit;
                     }
@@ -577,7 +633,7 @@ lep_decode_g2_kernel(const ImageDesc* __restrict__ images, SegDesc* __restrict__
                     const bool nbusy = bit ? b1 : b0;
                     uint32_t mwn = nbusy ? *g2_word(hot, model, mwidth, naddr) : 0u;
                     // ---- in the shadow of that load
-                    const uint32_t neww = g2_model_word(mw, bit);
+                    const uint32_t neww = g2_next_word(br, mw, bit);
                     *g2_word(hot, model, mwidth, addr) = (uint16_t)neww;
                     if (naddr == addr) mwn = neww;                 // saturated threshold index: the same branch twice in a row
                     g2_update(br, split, bit);
@@ -722,7 +778,7 @@ lep_decode_g2_kernel(const ImageDesc* __restrict__ images, SegDesc* __restrict__
                     const uint32_t naddr = bit ? a1 : a0;
                     const bool nbusy = bit ? b1 : b0;
                     uint32_t mwn = nbusy ? *g2_word(hot, model, mwidth, naddr) : 0u;
-                    const uint32_t neww = g2_model_word(mw, bit);
+                    const uint32_t neww = g2_next_word(br, mw, bit);
                     *g2_word(hot, model, mwidth, addr) = (uint16_t)neww;
                     if (naddr == addr) mwn = neww;
                     g2_update(br, split, bit);

@@ -591,6 +591,7 @@ struct DChunk {
     std::vector<lepb200_stream> streams;
     std::vector<lepb200_buffer> spans;          // mux packets of all streams of the chunk, in stream order
     std::vector<uint32_t> span_first;           // per stream: its first packet in `spans` (+ one past the end)
+    std::vector<uint8_t> coders;                // per batch image: LEPB200_CODER_ANS for a version-3 container, else LEPB200_CODER_BOOL
     std::vector<int32_t> seg_status;
     std::vector<int> seg_base;
     std::vector<lepb200_henc_image> henc;       // per batch image: scan re-encoded on the device when scan_bytes != 0
@@ -752,6 +753,7 @@ void decompress_front(DecompressCall& x, int k) {
             for (int t = 0; t < j.ncmp; ++t) { s.planes[i][t] = reinterpret_cast<int16_t*>(p); p += (plane_bytes(j, t) + 255) & ~size_t(255); }
         }
         fill_image(s.imgs[q], j, s.planes[i].data(), lf.handoffs);
+        s.coders.push_back(lf.version == 3 ? LEPB200_CODER_ANS : LEPB200_CODER_BOOL);
         // files that stay on the device have no host planes; the batch builder only wants the pointers non-null
         for (int t = 0; t < j.ncmp; ++t) if (!s.imgs[q].planes[t]) s.imgs[q].planes[t] = reinterpret_cast<int16_t*>(uintptr_t(1));
         for (int t = 0; t < lf.nseg; ++t) {
@@ -777,7 +779,8 @@ void decompress_gpu(DecompressCall& x, int k) {
     DChunk& s = x.cs[k];
     lepb200_ctx* ctx = x.run.ctx(k);
     if (s.gpu_rc == 0 && !s.imgs.empty()) {
-        s.gpu_rc = lepb200_decode_upload_gather(ctx, s.imgs.data(), (int)s.imgs.size(), s.streams.data(), s.spans.data(), s.span_first.data());
+        s.gpu_rc = lepb200_decode_upload_gather_coded(ctx, s.imgs.data(), (int)s.imgs.size(), s.streams.data(), s.spans.data(), s.span_first.data(),
+                                                      s.coders.data());
         x.run.mark("pack+upload", k, t0);
         if (s.gpu_rc == 0) s.gpu_rc = lepb200_decode_launch(ctx);
         const int parts = s.imgs.size() >= 256 ? x.henc_parts : 1;
@@ -1055,6 +1058,7 @@ size_t lepb200_host_generic_lep(const uint8_t* data, size_t len, uint8_t* out, s
     return lep.size();
 }
 int lepb200_host_lep_zlib0(const lepb200_lep* h) { return h && h->lf.zlib0 ? 1 : 0; }
+int lepb200_host_lep_coder(const lepb200_lep* h) { return h && h->lf.version == 3 ? LEPB200_CODER_ANS : LEPB200_CODER_BOOL; }
 size_t lepb200_host_zlib0_frame(const uint8_t* data, size_t len, uint8_t* out, size_t cap) {
     if (!data && len) return 0;
     const size_t need = zlib0_size(len);

@@ -91,7 +91,8 @@ inline uint32_t token_slot(unsigned long long bound) {
 struct BatchPlan {
     std::vector<ImageDesc> images;        // plane[c]: offset in the plane arena
     std::vector<SegDesc> segs;            // stream: offset in the stream arena; tokens: offset in the token arena (tokens_known)
-    std::vector<int> order;               // largest segments first
+    std::vector<int> order;               // bool-coded segments, then rANS-coded ones (decode), each part largest first
+    int order_ans = 0;                    // decode: order[order_ans ..] are the rANS-coded segments (CODER_ANS)
     std::vector<size_t> seg_blocks;       // blocks each segment codes
     std::vector<size_t> plane_bytes;      // per image * 3 + component
     size_t plane_total = 0, stream_total = 0, row_stride = 0;
@@ -100,9 +101,11 @@ struct BatchPlan {
 };
 
 // Job tables of an encode (in = nullptr) or decode batch (in = one stream per segment): ImageDesc / SegDesc, the plane arena
-// (256-byte aligned planes), the stream arena, the row stride of the kernels' row buffers and the launch order.
+// (256-byte aligned planes), the stream arena, the row stride of the kernels' row buffers and the launch order.  coders
+// (decode, optional): the entropy coder of each image's streams (LEPB200_CODER_BOOL / LEPB200_CODER_ANS); nullptr = all bool.
 // Returns nullptr, or what is wrong with the batch.
-inline const char* plan_batch(BatchPlan& b, const lepb200_image* images, int nimages, bool encode, const lepb200_stream* in) {
+inline const char* plan_batch(BatchPlan& b, const lepb200_image* images, int nimages, bool encode, const lepb200_stream* in,
+                              const uint8_t* coders = nullptr) {
     if (nimages <= 0 || !images) return "empty batch";
     b.images.assign(nimages, ImageDesc());
     b.segs.clear(); b.seg_blocks.clear(); b.plane_bytes.assign((size_t)nimages * 3, 0);
@@ -113,9 +116,11 @@ inline const char* plan_batch(BatchPlan& b, const lepb200_image* images, int nim
     for (int i = 0; i < nimages; ++i) {
         const lepb200_image& im = images[i];
         if (const char* e = validate_image(im)) return e;
+        if (coders && (encode || coders[i] > LEPB200_CODER_ANS)) return "invalid entropy coder";
         ImageDesc& d = b.images[i];
         memset(&d, 0, sizeof(d));
         d.ncmp = im.ncmp; d.mcuv = im.mcuv;
+        d.coder = coders && coders[i] == LEPB200_CODER_ANS ? CODER_ANS : CODER_BOOL;
         int qstatus = 0;
         size_t rs = 0;
         for (int c = 0; c < im.ncmp; ++c) {
@@ -163,11 +168,16 @@ inline const char* plan_batch(BatchPlan& b, const lepb200_image* images, int nim
             b.segs.push_back(sd);
         }
     }
-    // largest segments first (longest-processing-time-first on the persistent warps)
+    // largest segments first (longest-processing-time-first on the persistent warps); a decode kernel launch takes the
+    // segments of one coder, so those of the rANS coder follow all the others
     const int nseg = (int)b.segs.size();
     b.order.resize(nseg);
     for (int i = 0; i < nseg; ++i) b.order[i] = i;
-    std::stable_sort(b.order.begin(), b.order.end(), [&](int x, int y) { return b.seg_blocks[x] > b.seg_blocks[y]; });
+    auto coder = [&](int x) { return b.images[b.segs[x].image].coder; };
+    std::stable_sort(b.order.begin(), b.order.end(), [&](int x, int y) {
+        return coder(x) != coder(y) ? coder(x) < coder(y) : b.seg_blocks[x] > b.seg_blocks[y]; });
+    b.order_ans = nseg;
+    while (b.order_ans > 0 && coder(b.order[b.order_ans - 1]) == CODER_ANS) --b.order_ans;
     return nullptr;
 }
 
