@@ -122,6 +122,9 @@ int lepb200_encode_token_canaries(lepb200_ctx* ctx, uint8_t* moved, uint64_t* ch
 int lepb200_decode_upload(lepb200_ctx* ctx, const lepb200_image* images, int nimages, const lepb200_stream* in);
 int lepb200_decode_launch(lepb200_ctx* ctx);
 int lepb200_decode_fetch(lepb200_ctx* ctx, const lepb200_image* images, int nimages, int32_t* status_out);
+/* Per-segment decision counts of the batch the last lepb200_decode_fetch returned (out: one per segment, in batch order):
+ * the decisions each segment's decode took before it ended, well or not.  LEPB200_ERR_INVALID before that fetch. */
+int lepb200_decode_fetch_decisions(lepb200_ctx* ctx, uint64_t* out);
 
 /* Wait for everything queued on the context's stream. */
 int lepb200_sync(lepb200_ctx* ctx);

@@ -68,6 +68,7 @@ _EXPORTS = [
     "lepb200_host_lep_members", "lepb200_host_lep_open_member", "lepb200_encode_upload_tokens", "lepb200_encode_token_canaries", "lepb200_last_huffman_redone",
     "lepb200_codec_set_permissive", "lepb200_host_generic_lep", "lepb200_host_lep_generic",
     "lepb200_decode_upload_coded", "lepb200_decode_upload_gather_coded", "lepb200_host_lep_coder",
+    "lepb200_decode_fetch_decisions",
 ]
 
 CODER_BOOL, CODER_ANS = 0, 1          # LEPB200_CODER_*: bool coder (container versions 1, 2, 4), rANS coder (version 3)
@@ -108,6 +109,8 @@ def lib():
     L.lepb200_decode_upload_coded.restype = ctypes.c_int
     L.lepb200_decode_launch.argtypes = [vp]
     L.lepb200_decode_fetch.argtypes = [vp, ip, ctypes.c_int, ctypes.POINTER(ctypes.c_int32)]
+    L.lepb200_decode_fetch_decisions.argtypes = [vp, ctypes.POINTER(ctypes.c_uint64)]
+    L.lepb200_decode_fetch_decisions.restype = ctypes.c_int
     for f in ("lepb200_encode_images", "lepb200_encode_upload", "lepb200_encode_launch", "lepb200_encode_fetch",
               "lepb200_decode_images", "lepb200_decode_upload", "lepb200_decode_launch", "lepb200_decode_fetch",
               "lepb200_device_available"):
@@ -290,6 +293,13 @@ class LeptonB200Codec:
                         c[i].planes[k] = None
         self._check(self._L.lepb200_decode_fetch(self._ctx, c, len(self._dec_imgs), st), "decode_fetch")
         return list(st)
+
+    def decode_decisions(self):
+        """Per-segment decision counts of the batch the last decode_fetch returned: where each segment's decode ended."""
+        n = sum(im.nseg for im in self._dec_imgs)
+        nd = (ctypes.c_uint64 * n)()
+        self._check(self._L.lepb200_decode_fetch_decisions(self._ctx, nd), "decode_decisions")
+        return list(nd)
 
     def decode_images(self, images, streams, coders=None):
         """Decodes into ``images[i].planes`` (pre-allocated).  Returns per-segment status codes.  coders: per image,

@@ -96,6 +96,7 @@ struct lepb200_ctx {
     std::vector<int> rc_redo;             // serial range coder: segments it codes again
     int grid = 0;
     bool have_batch = false, launched = false, symbolised = false, is_encode = true;
+    bool decode_fetched = false;          // h_segs holds the segment records of the current decode batch (lepb200_decode_fetch)
     float last_ms = -1.f, last_ms_a = -1.f, last_ms_huff = -1.f;
     uint64_t launches = 0;
     uint64_t alg_bytes = 0;
@@ -211,7 +212,7 @@ template <class WarpReader, class GroupCoder> int decode_launch_part(lepb200_ctx
 // Common part of encode/decode upload: job tables (lep_plan.cuh), launch shape, pools, upload of the tables.
 int build_batch(lepb200_ctx* ctx, const lepb200_image* images, int nimages, bool encode, const lepb200_stream* in,
                 const uint8_t* coders = nullptr) {
-    ctx->have_batch = false; ctx->launched = false; ctx->is_encode = encode; ctx->canary = false;
+    ctx->have_batch = false; ctx->launched = false; ctx->is_encode = encode; ctx->canary = false; ctx->decode_fetched = false;
     BatchPlan& b = ctx->batch;
     if (const char* e = plan_batch(b, images, nimages, encode, in, coders)) { ctx->err = e; return LEPB200_ERR_INVALID; }
     const int nseg = (int)b.segs.size();
@@ -370,7 +371,7 @@ void lepb200_release_device_buffers(lepb200_ctx* ctx) {
                       &ctx->d_henc_imgs, &ctx->d_henc_segs, &ctx->d_henc_tabs, &ctx->d_gather, &ctx->d_lit, &ctx->d_rc_ck, &ctx->d_rc_digits,
                       &ctx->d_rc_ovf, &ctx->d_rc_redo})
         b->release();
-    ctx->have_batch = ctx->launched = false;
+    ctx->have_batch = ctx->launched = ctx->decode_fetched = false;
 }
 
 const char* lepb200_last_error(const lepb200_ctx* ctx) { return ctx ? ctx->err.c_str() : "null context"; }
@@ -467,7 +468,7 @@ int lepb200_huffman_stage_upload(lepb200_ctx* ctx, size_t offset, size_t bytes) 
 int lepb200_huffman_decode_to_device(lepb200_ctx* ctx, lepb200_jpeg_scan* scans, int n) {
     if (!ctx || !scans || n <= 0) return LEPB200_ERR_INVALID;
     CK(cudaSetDevice(ctx->device));
-    ctx->have_batch = false; ctx->launched = false; ctx->resident_images = 0;
+    ctx->have_batch = false; ctx->launched = false; ctx->decode_fetched = false; ctx->resident_images = 0;
     // sub-sequence length of the many-threads-per-image kernels: longer sub-sequences need fewer synchronisation passes
     // (8192 bits: 3, 4096: 5, 2048: 9 on 1080p files), as long as the batch still gives every SM its 2048 threads
     int sub_bits = ctx->huff_sub_bits;
@@ -846,7 +847,7 @@ int lepb200_encode_upload_tokens(lepb200_ctx* ctx, const uint16_t* tokens, const
                                  const int32_t* seg_per_file, int nfiles) {
     if (!ctx || !tokens || !ntok || !caps || nseg <= 0 || !seg_per_file || nfiles <= 0) return LEPB200_ERR_INVALID;
     CK(cudaSetDevice(ctx->device));
-    ctx->have_batch = ctx->launched = ctx->symbolised = false; ctx->is_encode = true; ctx->canary = true;
+    ctx->have_batch = ctx->launched = ctx->symbolised = ctx->decode_fetched = false; ctx->is_encode = true; ctx->canary = true;
     BatchPlan& b = ctx->batch;
     b.images.assign(nfiles, ImageDesc());
     b.segs.assign(nseg, SegDesc());
@@ -1159,6 +1160,7 @@ int lepb200_decode_launch(lepb200_ctx* ctx) {
     CK(cudaSetDevice(ctx->device));
     const int nseg = (int)ctx->batch.segs.size();
     const int nbool = ctx->batch.order_ans;
+    ctx->decode_fetched = false;
     CK(cudaMemsetAsync(ctx->d_counter.p, 0, sizeof(int), ctx->stream));
     CK(cudaEventRecord(ctx->ev0, ctx->stream));
     int r = nbool > 0 ? decode_launch_part<BoolReader, G2Bool>(ctx, 0, nbool, ctx->dec_threads, ctx->dec_group_grid, ctx->grid) : LEPB200_OK;
@@ -1192,6 +1194,14 @@ int lepb200_decode_fetch(lepb200_ctx* ctx, const lepb200_image* images, int nima
         alg += (uint64_t)ctx->batch.seg_blocks[s] * 128 + ctx->batch.segs[s].cap;
     }
     ctx->alg_bytes = alg;
+    ctx->decode_fetched = true;
+    return LEPB200_OK;
+}
+
+int lepb200_decode_fetch_decisions(lepb200_ctx* ctx, uint64_t* out) {
+    if (!ctx || !out || !ctx->decode_fetched) { if (ctx) ctx->err = "decode_fetch_decisions without decode_fetch"; return LEPB200_ERR_INVALID; }
+    const SegDesc* hs = static_cast<const SegDesc*>(ctx->h_segs.p);
+    for (size_t s = 0; s < ctx->batch.segs.size(); ++s) out[s] = (uint64_t)hs[s].ndecisions_lo | ((uint64_t)hs[s].ndecisions_hi << 32);
     return LEPB200_OK;
 }
 

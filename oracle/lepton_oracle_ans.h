@@ -89,9 +89,22 @@ int lo_ans_encode(const uint16_t *tokens, size_t n, uint8_t *out, size_t cap, si
     return 0;
 }
 
+/* One decision of a decode, as lo_decode_segment_ans_trace records it (test infrastructure: to build streams whose
+ * decisions land on chosen states, and to show that a corpus reaches an edge of the coder). */
+typedef struct {
+    uint64_t x_before;                     /* the state the decision reads (its low byte against the probability) */
+    uint64_t x_after;                      /* that state advanced, refilled when it fell below 2^31: the state two decisions on */
+    int64_t word_off;                      /* byte offset in the stream of the word the refill took; -1: no refill */
+    uint8_t prob, bit;                     /* the model's probability, the decoded bit */
+    uint8_t c0, c1;                        /* the branch counts before the update (1..255) */
+    uint8_t pad[4];
+} lo_ans_step;
+
 /* the coder of the segment in progress */
 static struct {
     AnsReader ar;                          /* decode */
+    const uint8_t *base;                   /* decode: start of the stream */
+    lo_ans_step *trace; size_t ntrace, trace_cap;   /* decode, optional: the first trace_cap decisions */
     uint16_t *tok; size_t ntok, tok_cap;   /* encode: the decisions (prob | bit << 8), coded at the end in reverse */
 } g_ans;
 
@@ -103,6 +116,15 @@ static inline int code_bit(Codec *c, Branch *b, int bit) {
             g_ans.tok = (uint16_t *)realloc(g_ans.tok, g_ans.tok_cap * sizeof(uint16_t));
         }
         g_ans.tok[g_ans.ntok++] = (uint16_t)(b->p | bit << 8);
+    } else if (g_ans.ntrace < g_ans.trace_cap) {
+        lo_ans_step *t = &g_ans.trace[g_ans.ntrace++];
+        const uint8_t *p0 = g_ans.ar.p;
+        t->x_before = g_ans.ar.x0;
+        t->prob = b->p; t->c0 = b->c0; t->c1 = b->c1;
+        bit = ar_read(&g_ans.ar, b->p);
+        t->bit = (uint8_t)bit;
+        t->x_after = g_ans.ar.x1;
+        t->word_off = g_ans.ar.p != p0 ? (int64_t)(p0 - g_ans.base) : -1;
     } else {
         bit = ar_read(&g_ans.ar, b->p);
     }

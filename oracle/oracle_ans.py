@@ -28,6 +28,8 @@ def lib():
         L.lo_decode_segment_ans.argtypes = [ctypes.POINTER(Geometry), P3, ctypes.c_int, ctypes.c_int, ctypes.c_int,
                                             ctypes.c_void_p, ctypes.c_size_t, ctypes.POINTER(ctypes.c_uint64)]
         L.lo_decode_segment_ans.restype = ctypes.c_int
+        L.lo_decode_segment_ans_trace.argtypes = L.lo_decode_segment_ans.argtypes + [ctypes.c_void_p, ctypes.c_size_t]
+        L.lo_decode_segment_ans_trace.restype = ctypes.c_int
         L.lo_ans_encode.argtypes = [ctypes.c_void_p, ctypes.c_size_t, ctypes.c_void_p, ctypes.c_size_t, ctypes.POINTER(ctypes.c_size_t)]
         L.lo_ans_encode.restype = ctypes.c_int
         _LIB = L
@@ -52,6 +54,28 @@ def decode_segment(g: Geometry, planes, min_y, max_y, is_last, stream: bytes):
     rc = lib().lo_decode_segment_ans(ctypes.byref(g), _ptrs(planes), min_y, max_y, int(is_last),
                                      buf.ctypes.data if len(buf) else None, len(buf), ctypes.byref(nd))
     return rc, nd.value
+
+
+# lo_ans_step (lepton_oracle_ans.h): one decision of a decode
+TRACE_DTYPE = np.dtype([("x_before", "<u8"), ("x_after", "<u8"), ("word_off", "<i8"), ("prob", "u1"), ("bit", "u1"),
+                        ("c0", "u1"), ("c1", "u1"), ("pad", "u1", 4)])
+assert TRACE_DTYPE.itemsize == 32
+
+
+def decode_segment_trace(g: Geometry, planes, min_y, max_y, is_last, stream: bytes):
+    """decode_segment with a record of every decision -> (exit_code, ndecisions, trace): trace is a TRACE_DTYPE array, one
+    entry per decision: the probability, the bit, the branch counts before the update (c0, c1), the state the decision
+    reads (x_before) and that state advanced and refilled (x_after), and the stream offset of the word the refill took
+    (word_off, -1 without a refill)."""
+    rc, nd = decode_segment(g, planes, min_y, max_y, is_last, stream)     # sizes the trace; decoding again writes the same
+    buf = np.frombuffer(stream, dtype=np.uint8)
+    trace = np.zeros(max(nd, 1), TRACE_DTYPE)
+    n = ctypes.c_uint64(0)
+    rc2 = lib().lo_decode_segment_ans_trace(ctypes.byref(g), _ptrs(planes), min_y, max_y, int(is_last),
+                                            buf.ctypes.data if len(buf) else None, len(buf), ctypes.byref(n),
+                                            trace.ctypes.data, len(trace))
+    assert (rc2, n.value) == (rc, nd)
+    return rc, nd, trace[:nd]
 
 
 def ans_encode(tokens, cap=None):

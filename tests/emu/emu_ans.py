@@ -30,9 +30,10 @@ def lib():
     return _LIB
 
 
-def decode_images(kernel, images, streams, coders, grid_cap=0, reverse=False):
+def decode_images(kernel, images, streams, coders, grid_cap=0, reverse=False, kernel_ans=None):
     """emu.decode_images with the entropy coder of every image's streams (CODER_BOOL, CODER_ANS): decodes into
-    images[i].planes, returns (status, ndecisions) per segment."""
+    images[i].planes, returns (status, ndecisions) per segment.  kernel_ans: the kernel of the rANS-coded segments'
+    launch (default: `kernel`)."""
     from lepton_b200.codec import _Image, _Stream
     assert len(coders) == len(images)
     n = sum(im.nseg for im in images)
@@ -50,7 +51,7 @@ def decode_images(kernel, images, streams, coders, grid_cap=0, reverse=False):
     cod = (ctypes.c_uint8 * len(images))(*[int(c) for c in coders])
     st = (ctypes.c_int32 * n)()
     nd = (ctypes.c_uint64 * n)()
-    rc = lib().emu_decode_images_coded(int(kernel), int(grid_cap), int(bool(reverse)), cim, len(images), arr, cod, st, nd)
+    rc = lib().emu_decode_images_coded(int(kernel), -1 if kernel_ans is None else int(kernel_ans), int(grid_cap), int(bool(reverse)), cim, len(images), arr, cod, st, nd)
     if rc != 0:
         raise RuntimeError("emu_decode_images_coded failed with %d" % rc)
     return list(st), list(nd)

@@ -68,12 +68,13 @@ void group_shape(int G, int& warps, int& per_warp) {
 // like the device arena); per-segment status and decision counts come back like lepb200_decode_fetch reports them.
 // reverse = 1 runs the launch's CTAs and threads in reverse order (emu::g_reverse).  coders (optional): the entropy coder of
 // each image's streams (LEPB200_CODER_*); as in lepb200_decode_launch, the bool-coded segments of the batch are decoded by one
-// launch and the rANS-coded ones by another, both of the given kernel.
-extern "C" int emu_decode_images_coded(int kernel, int grid_cap, int reverse, const lepb200_image* images, int nimages, const lepb200_stream* in,
-                                       const uint8_t* coders, int32_t* status_out, uint64_t* ndecisions_out) {
-    const int gl = kernel % 100;
-    const bool group = kernel / 100 == 2 && (gl == 1 || gl == 2 || gl == 4 || gl == 8 || gl == 16 || gl == 32);
-    if (!in || (kernel != 0 && !group)) return LEPB200_ERR_INVALID;
+// launch and the rANS-coded ones by another: of the given kernel, or the rANS-coded ones of kernel_ans (>= 0), so that the
+// two parts of a batch can take different kernels as the library's size switch gives them.
+extern "C" int emu_decode_images_coded(int kernel, int kernel_ans, int grid_cap, int reverse, const lepb200_image* images, int nimages,
+                                       const lepb200_stream* in, const uint8_t* coders, int32_t* status_out, uint64_t* ndecisions_out) {
+    auto is_group = [](int k) { const int gl = k % 100; return k / 100 == 2 && (gl == 1 || gl == 2 || gl == 4 || gl == 8 || gl == 16 || gl == 32); };
+    if (kernel_ans < 0) kernel_ans = kernel;
+    if (!in || (kernel != 0 && !is_group(kernel)) || (kernel_ans != 0 && !is_group(kernel_ans))) return LEPB200_ERR_INVALID;
     BatchPlan b;
     if (plan_batch(b, images, nimages, false, in, coders)) return LEPB200_ERR_INVALID;
     const int nseg = (int)b.segs.size();
@@ -87,8 +88,10 @@ extern "C" int emu_decode_images_coded(int kernel, int grid_cap, int reverse, co
     for (int part = 0; part < 2; ++part) {
         const int first = part == 0 ? 0 : b.order_ans, n = part == 0 ? b.order_ans : nseg - b.order_ans;
         if (n == 0) continue;
+        const int kernel_part = part == 0 ? kernel : kernel_ans;
+        const bool group = is_group(kernel_part);
         LaunchArgs a;
-        a.kernel = kernel; a.ans = part == 1; a.images = b.images.data(); a.segs = segs.data(); a.nseg = n; a.order = b.order.data() + first;
+        a.kernel = kernel_part; a.ans = part == 1; a.images = b.images.data(); a.segs = segs.data(); a.nseg = n; a.order = b.order.data() + first;
         a.row_stride = b.row_stride;
         int counter = 0;
         a.counter = &counter;
@@ -97,7 +100,7 @@ extern "C" int emu_decode_images_coded(int kernel, int grid_cap, int reverse, co
         if (group) {
             // 200 + G: lep_decode_g2_kernel<G>; grid_cap > 0 limits the CTAs so that groups take several segments from the queue
             int warps, per_warp;
-            group_shape(kernel % 100, warps, per_warp);
+            group_shape(kernel_part % 100, warps, per_warp);
             grid = (unsigned)((n + warps * per_warp - 1) / (warps * per_warp));
             if (grid_cap > 0) grid = std::min(grid, (unsigned)grid_cap);
             block = (unsigned)warps * 32;
@@ -107,8 +110,8 @@ extern "C" int emu_decode_images_coded(int kernel, int grid_cap, int reverse, co
             if (grid_cap > 0) grid = std::min(grid, (unsigned)grid_cap);
             block = DEC_WARPS_PER_CTA * 32;
         }
-        const size_t slots = kernel == 0 ? (size_t)grid * DEC_WARPS_PER_CTA : (size_t)n;
-        std::vector<uint16_t> models(slots * M_TOTAL, kernel == 0 ? 0x5a5a : 0);       // thread / group kernels: zero fill before the launch; the warp kernel clears its own
+        const size_t slots = kernel_part == 0 ? (size_t)grid * DEC_WARPS_PER_CTA : (size_t)n;
+        std::vector<uint16_t> models(slots * M_TOTAL, kernel_part == 0 ? 0x5a5a : 0);       // thread / group kernels: zero fill before the launch; the warp kernel clears its own
         std::vector<uint8_t> rows((group ? group_slots : slots) * b.row_stride, 0);
         a.models = models.data(); a.rows = rows.data();
         emu::g_reverse = reverse != 0;

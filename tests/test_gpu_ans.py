@@ -1,7 +1,8 @@
 """Container version 3 (the reference's -ans files: rANS-coded streams) on the GPU: the decode kernels through the C ABI,
 and the file API and the CLI against what the reference restored from every fixture of tests/golden/ans.json
-(tests/golden/make_ans.py)."""
+(tests/golden/make_ans.py) and from damaged ones (tests/golden/ans_damaged.json, tests/golden/make_ans_damaged.py)."""
 import hashlib
+import json
 import os
 import subprocess
 import zlib
@@ -190,3 +191,36 @@ def test_cli_single_file_and_batch_mode(key, tmp_path):
             assert md5((outdir / outs[0]).read_bytes()) == restore_want(n, key)[1], n
     else:
         assert r.returncode != 0
+
+
+DAMAGED = json.load(open(os.path.join(GOLDEN, "ans_damaged.json")))
+
+
+def test_damaged_files_restore_like_the_reference():
+    """Version-3 fixtures with stream bytes of their mux packets damaged, and their version-1 twins damaged at the same
+    segment and stream offsets, all in one call of the file API: each ends with the reference's exit code, and where that
+    is 0, with the bytes it wrote (their md5).  Without libbrotlidec every version-3 file is refused with 200."""
+    from lepton_b200 import LeptonB200FileCodec
+    names = sorted(DAMAGED["cases"])
+    inputs = []
+    for n in names:
+        e = DAMAGED["cases"][n]
+        b = bytearray(open(os.path.join(ANS_DIR, e["fixture"]), "rb").read())
+        for off, x in e["flips"]:
+            b[off] ^= x
+        assert md5(b) == e["input_md5"], n
+        inputs.append(bytes(b))
+    assert sum(1 for n in names if not n.endswith(".v1")) >= 15 and any(DAMAGED["cases"][n]["rc"] == 0 for n in names)
+    fc = LeptonB200FileCodec(0, host_threads=8)
+    try:
+        got = fc.decompress(inputs)
+    finally:
+        fc.close()
+    have = brotli_available()
+    wrong = []
+    for n, (s, b) in zip(names, got):
+        e = DAMAGED["cases"][n]
+        want = (e["rc"], e["md5"]) if have or n.endswith(".v1") else (200, None)
+        if (s, md5(b) if s == 0 else None) != want:
+            wrong.append((n, s, want[0]))
+    assert not wrong, wrong

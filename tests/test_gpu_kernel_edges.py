@@ -6,8 +6,9 @@ range pass and its prologue, the plain stores and atomic adds of piece CTAs that
 queues shared by CTAs that run together, the group kernel's shared-memory front region at two CTAs per SM, and the
 batch-size switches of the token feed and of the decode kernel.
 
-Expected values come from the oracle (oracle.bool_encode, oracle.decode_segment) or from the host writer's mux plan
-(lepb200_host_mux_plan); the inputs are the emulator tests' own builders.
+Expected values come from the oracle (oracle.bool_encode, oracle.decode_segment, and oracle_ans for the rANS coder of
+container version 3) or from the host writer's mux plan (lepb200_host_mux_plan); the inputs are the emulator tests' own
+builders.
 """
 import functools
 import os
@@ -22,6 +23,7 @@ import oracle  # noqa: E402
 import test_emu_decode_lookahead as lookahead  # noqa: E402
 import test_emu_model_interleave as interleave  # noqa: E402
 import test_emu_rangecoder as rangecoder  # noqa: E402
+from ans_helpers import judge, oracle_ans_streams, traces  # noqa: E402
 from helpers import oracle_encode_image, random_coef_image  # noqa: E402
 from test_emu_rangecoder import carry_tokens, random_tokens, tok  # noqa: E402
 
@@ -156,27 +158,29 @@ def test_gather_assembles_the_host_writers_files(monkeypatch, seed):
 
 
 # ---------------------------------------------------------------------------------------------------- decode
-def decode_vs_oracle(codec, imgs, streams, want_rc=None):
-    """Decodes `streams` for `imgs` in one batch: per-segment statuses must be the oracle's return codes (want_rc, default
-    all 0), and every image whose segments all decode cleanly (or, damaged, with status 0) must hold the oracle's planes."""
-    from lepton_b200 import CoefImage
-    from helpers import oracle_decode_image
-    out = [CoefImage(ncmp=i.ncmp, mcuv=i.mcuv, bch=i.bch, bcv=i.bcv, qtables_zigzag=i.qtables_zigzag,
-                     planes=[np.full_like(p, -5) for p in i.planes], luma_y_start=i.luma_y_start, trunc_bcv=i.trunc_bcv,
-                     trunc_bc=i.trunc_bc) for i in imgs]
-    st = codec.decode_images(out, streams)
-    n = sum(i.nseg for i in imgs)
-    assert st == (want_rc or [0] * n), [(k, a, b) for k, (a, b) in enumerate(zip(st, want_rc or [0] * n)) if a != b][:8]
-    k = 0
-    for i, (img, o, ss) in enumerate(zip(imgs, out, streams)):
-        if not any(st[k:k + img.nseg]):
-            want = oracle_decode_image(img, ss)
-            for c in range(img.ncmp):
-                assert np.array_equal(o.planes[c], want[c]), (i, c)
-        k += img.nseg
+# Every decode batch below runs once with bool-coded streams (container versions 1, 2, 4) and once with rANS-coded ones
+# (version 3): same grammar and batches, the other coder's kernels, judged against that coder's oracle.
+BOOL, ANS = 0, 1
+CODERS = {"bool": BOOL, "ans": ANS}
 
 
-def oracle_streams(imgs):
+def device_run(codec):
+    """ans_helpers.judge's run on a context: -> (status, decision count) of every segment"""
+    def run(out, streams, coders):
+        st = codec.decode_images(out, streams, coders)
+        return st, codec.decode_decisions()
+    return run
+
+
+def decode_vs_oracle(codec, imgs, streams, coder=BOOL, refused=()):
+    """Decodes `streams` for `imgs` in one batch of one coder (bool: the entry point without a coder argument): status,
+    decision count and planes of every segment are the oracle's.  -> the oracle's statuses"""
+    return judge(device_run(codec), imgs, streams, None if coder == BOOL else [coder] * len(imgs), refused)
+
+
+def oracle_streams(imgs, coder=BOOL):
+    if coder == ANS:
+        return oracle_ans_streams(imgs)
     refs = [oracle_encode_image(img) for img in imgs]
     for r in refs:
         assert all(rc == 0 for rc, _, _ in r)
@@ -190,25 +194,37 @@ def decoder(request, monkeypatch):
     c.close()
 
 
+@pytest.fixture(params=list(CODERS))
+def coder(request):
+    return CODERS[request.param]
+
+
 @pytest.mark.parametrize("batch", lookahead.HAZARD_BATCHES, ids=lambda f: f.__name__)
-def test_read_ahead_hazard_batches(decoder, batch):
+def test_read_ahead_hazard_batches(decoder, batch, coder):
+    """With the rANS coder the special-state batch is the saturate-and-restart case: its all-ones sign branch counts
+    up to c1 = 255, restarts at 129 and decides at probability 1 (the rANS model has no special state)."""
     imgs, _ = batch()
-    decode_vs_oracle(decoder, imgs, oracle_streams(imgs))
+    streams = oracle_streams(imgs, coder)
+    if coder == ANS and batch is lookahead.special_state_batch:
+        t = traces(imgs, streams)
+        assert np.any((t["c0"] == 1) & (t["c1"] == 255) & (t["bit"] == 1))
+        assert np.any((t["c1"] == 129) & (t["prob"] < 128)) and np.any(t["prob"] == 1)
+    decode_vs_oracle(decoder, imgs, streams, coder)
 
 
 @pytest.mark.parametrize("spec", [interleave.PARTIAL_BLOCK, interleave.SECOND_CLAIMS], ids=["partial_block", "second_claims"])
-def test_interleave_batches(decoder, spec):
+def test_interleave_batches(decoder, spec, coder):
     sizes, seed, _ = spec
     imgs, streams, want = interleave.batch(sizes, seed)
-    st = decoder.decode_images(imgs, streams)
-    assert st == [0] * sum(sizes)
     for img, (planes, _) in zip(imgs, want):
-        for c in range(img.ncmp):
-            assert np.array_equal(img.planes[c], planes[c])
+        img.planes = planes
+    if coder == ANS:
+        streams = oracle_ans_streams(imgs)
+    decode_vs_oracle(decoder, imgs, streams, coder)
 
 
 @functools.lru_cache(maxsize=None)
-def small_segments(n, seed=31):
+def small_segments(n, coder=BOOL, seed=31):
     """Images of 1..16 one-row segments, n segments in all, with their oracle streams."""
     rng = np.random.default_rng(seed + n)
     imgs, streams, left = [], [], n
@@ -217,20 +233,21 @@ def small_segments(n, seed=31):
         img = random_coef_image(rng, ncmp=1, mcuh=int(rng.integers(1, 4)), mcuv=nseg, sf=((1, 1),), nseg=nseg, density=0.4)
         imgs.append(img)
         left -= nseg
-    return imgs, oracle_streams(imgs)
+    return imgs, oracle_streams(imgs, coder)
 
 
 SEGMENT_COUNTS = list(range(1, 18)) + [23, 25, 63, 65, 255, 257, 1023, 1025, 6143, 6145, 6151, 6153]
 
 
 @pytest.mark.parametrize("n", SEGMENT_COUNTS)
-def test_segment_counts_of_every_residue_mod_8(monkeypatch, n):
+def test_segment_counts_of_every_residue_mod_8(monkeypatch, n, coder):
     """The batches below with the kernel the library picks itself: the warp kernel up to 6143 segments, the group kernel
-    at 4 lanes from 6144 on (6145, 6151 and 6153: a partial last warp and interleave block in one launch)."""
+    at 4 lanes from 6144 on (6145, 6151 and 6153: a partial last warp and interleave block in one launch).  A batch of
+    one coder is one part, so the switch applies to the rANS part alone as it does to the bool one."""
     c = codec_with(monkeypatch, {})
-    imgs, streams = small_segments(n)
+    imgs, streams = small_segments(n, coder)
     try:
-        decode_vs_oracle(c, imgs, streams)
+        decode_vs_oracle(c, imgs, streams, coder)
     finally:
         c.close()
 
@@ -246,37 +263,42 @@ ONE_LAUNCH_FORMS = {
 
 @pytest.mark.parametrize("n", [n for n in SEGMENT_COUNTS if n < 6144])
 @pytest.mark.parametrize("form", list(ONE_LAUNCH_FORMS))
-def test_segment_counts_of_every_residue_mod_8_on_every_kernel(monkeypatch, form, n):
+def test_segment_counts_of_every_residue_mod_8_on_every_kernel(monkeypatch, form, n, coder):
     """Batches whose segment count takes every residue mod 8 forced onto each kernel: in the group kernel, a last warp
     with 1..7 of its groups busy (at 4 lanes; 1..3 at 8 lanes) and a partial last interleave block of 1..7 models, in a
     pool of exactly n models; at 32 lanes, one segment per warp."""
     c = codec_with(monkeypatch, ONE_LAUNCH_FORMS[form])
-    imgs, streams = small_segments(n)
+    imgs, streams = small_segments(n, coder)
     try:
-        decode_vs_oracle(c, imgs, streams)
+        decode_vs_oracle(c, imgs, streams, coder)
     finally:
         c.close()
 
 
-def test_damaged_streams_next_to_healthy_ones(decoder):
+def test_damaged_streams_next_to_healthy_ones(decoder, coder):
     """48 one-segment images of one geometry (so the launch order is the batch order): every eighth segment from the
     third on is cut short and bit-flipped, so each warp of the group kernel and each interleave block of 8 models holds
-    one damaged segment among healthy ones.  Statuses are the oracle's return codes; the healthy neighbours' planes stay
-    exact."""
+    one damaged segment among healthy ones.  Statuses, decision counts and planes (those a failing segment wrote
+    included) are the oracle's.  rANS streams are cut to every length residue mod 4 and damaged in the 16 state bytes
+    as well as in the body, and one image with a zero quantiser is refused on the host (status 43) inside the batch."""
     rng = np.random.default_rng(41)
     imgs = [random_coef_image(rng, ncmp=3, mcuh=3, mcuv=2, sf=((2, 2), (1, 1), (1, 1)), nseg=1, density=0.6) for _ in range(48)]
-    streams = oracle_streams(imgs)
-    want_rc = []
-    for i, (img, ss) in enumerate(zip(imgs, streams)):
+    streams = oracle_streams(imgs, coder)
+    for i, ss in enumerate(streams):
         if i % 8 == 3:
             b = bytearray(ss[0][:max(8, len(ss[0]) // (2 + i % 5))])
+            if coder == ANS:
+                b = b[:len(b) - (len(b) - i // 8) % 4]               # lengths of residue 0, 1, 2, 3, 0, 1 mod 4
+            lo, hi = 4, len(b)
+            if coder == ANS:
+                lo, hi = (0, 16) if i // 8 % 2 else (16, len(b))    # the state bytes, or the body
             for _ in range(1 + i % 4):
-                b[int(rng.integers(4, len(b)))] ^= int(rng.integers(1, 256))
+                b[int(rng.integers(lo, min(hi, len(b))))] ^= int(rng.integers(1, 256))
             ss[0] = bytes(b)
-            g = oracle.make_geometry(img.ncmp, list(img.bch), list(img.bcv), img.mcuv, img.qtables_zigzag)
-            rc, _ = oracle.decode_segment(g, [np.zeros_like(p) for p in img.planes], 0, img.bcv[0], True, ss[0])
-            want_rc.append(rc)
-        else:
-            want_rc.append(0)
-    assert any(want_rc)
-    decode_vs_oracle(decoder, imgs, streams, want_rc)
+    refused = ()
+    if coder == ANS:
+        assert sorted({len(ss[0]) % 4 for i, ss in enumerate(streams) if i % 8 == 3}) == [0, 1, 2, 3]
+        imgs[21].qtables_zigzag = [[0] + list(q[1:]) for q in imgs[21].qtables_zigzag]
+        refused = (21,)
+    st = decode_vs_oracle(decoder, imgs, streams, coder, refused)
+    assert sum(1 for s in st if s) >= 3 + len(refused)

@@ -381,6 +381,36 @@ def test_corrupt_files_fail_alone_inside_a_batch():
     for n, (st, out), ref in zip(good, back[:4], good_jpg):
         assert st == 0 and out == ref, n
     assert all(st != 0 or len(out) > 0 for st, out in back[4:])
+    # version-3 (rANS) files: payload bytes flipped, the mux packets cut short, the brotli header blob damaged, next to
+    # intact version-3 and version-1 files of the same call
+    import hashlib
+    from ans_helpers import ANS, ANS_DIR
+    good_ans = ["iphonecrop2_t4", "colorswap", "geo_y22_odd", "all22_tall_t8"]
+    ans_lep = [open(os.path.join(ANS_DIR, n + ".lep"), "rb").read() for n in good_ans]
+    bad_ans = []
+    for k in range(24):
+        l = bytearray(ans_lep[k % 4])
+        zlen = int.from_bytes(l[24:28], "little")
+        body = 31 + zlen                                      # behind "CMP": the mux packets of the rANS streams
+        if k % 3 == 0:
+            for _ in range(1 + k % 4):
+                l[rnd.randrange(28, body)] = rnd.randrange(256)
+        elif k % 3 == 1:
+            for _ in range(1 + k % 4):
+                l[rnd.randrange(body, len(l) - 4)] ^= rnd.randrange(1, 256)
+        else:
+            l = l[:rnd.randrange(body, len(l) - 4)] + l[-4:]
+        bad_ans.append(bytes(l))
+    back = fc.decompress(ans_lep + good_lep[:2] + bad_ans)
+    from lepton_b200.codec import lib
+    for n, (st, out) in zip(good_ans, back[:4]):
+        if lib().lepb200_host_brotli_available():
+            assert st == 0 and hashlib.md5(out).hexdigest() == ANS[n]["restore"]["md5"], n
+        else:                                                 # no libbrotlidec: the header blob cannot be read
+            assert st == 200, n
+    for n, (st, out), ref in zip(good, back[4:6], good_jpg):
+        assert st == 0 and out == ref, n
+    assert all(st != 0 or len(out) > 0 for st, out in back[6:])
     # files that still compress must also restore exactly (a damaged scan is just another JPEG to the coder)
     again = [lep for st, lep in res[4:] if st == 0]
     src = [j for j, (st, _) in zip(bad_jpg, res[4:]) if st == 0]
