@@ -363,7 +363,8 @@ int lepb200_host_jpeg_open_embedded(const uint8_t* data, size_t len, int min_thr
 const char* lepb200_host_jpeg_error(const lepb200_jpeg* h);
 int lepb200_host_jpeg_image(lepb200_jpeg* h, lepb200_image* img);
 /* the scan as lepb200_huffman_decode_to_device takes it (de-stuffed entropy bytes, tables, geometry; pointers valid until
- * *_close; `rows` and the outputs are left alone); LEPB200_ERR_INVALID when the file needs the host Huffman decoder */
+ * *_close; `rows` and the outputs are left alone), also when the host Huffman decoder refused the scan, as the file API
+ * hands it to the device before any host decode; LEPB200_ERR_INVALID when the file needs the host Huffman decoder */
 int lepb200_host_jpeg_scan(lepb200_jpeg* h, lepb200_jpeg_scan* scan);
 int lepb200_host_jpeg_write_lep(lepb200_jpeg* h, const lepb200_stream* streams, int nseg, const uint8_t** data, size_t* len);
 /* everything of the .lep in front of the mux packets (what lepb200_encode_fetch_files wants as headers[i]) */

@@ -285,6 +285,7 @@ struct ChunkState {
     std::vector<std::array<int16_t*, 4>> planes;        // host planes of host-decoded files (else null)
     std::vector<Splits> splits;
     std::vector<uint8_t> host_decoded;                  // 1: planes came from the host Huffman decoder
+    std::vector<std::vector<int16_t>> redo_planes;      // planes of the files the device decoder left to the host
     std::vector<lepb200_image> imgs;                    // batch order == idx order
     std::vector<int> idx;                               // file index (relative to begin) of imgs[q]
     std::vector<lepb200_jpeg_scan> scans;               // per batch image
@@ -432,10 +433,24 @@ void select_segments(CompressCall& x, ChunkState& s) {
     lepb200_codec* c = x.c;
     const int nb = (int)s.idx.size();
     s.imgs.resize(nb);
+    s.redo_planes.assign(s.js.size(), std::vector<int16_t>());
     parallel_for(nb, x.run.pth(), [&](int q) {
         const int i = s.idx[q];
         Jpeg& j = *s.js[i];
         const lepb200_jpeg_scan& sc = s.scans[q];
+        if (!s.host_decoded[i] && sc.status == NOT_HANDLED) {
+            // the device decoder stops where the host decoder goes on (entropy data that ends inside a block, a zero run
+            // past the end of a block): the host decodes the file, and its planes go to the encoder as a placeholder's
+            size_t off[4] = {0, 0, 0, 0}, total = 0;
+            for (int t = 0; t < j.ncmp; ++t) { off[t] = total; total += plane_bytes(j, t) / 2; }
+            std::vector<int16_t>& store = s.redo_planes[i];
+            store.assign(total, 0);
+            for (int t = 0; t < j.ncmp; ++t) s.planes[i][t] = store.data() + off[t];
+            if (decode_scans(j, s.planes[i].data())) s.splits[i] = select_splits(j, c->max_encode_threads, c->min_encode_threads, c->even_split);
+            else s.splits[i].selected.assign(1, Handoff());
+            s.host_decoded[i] = 1;
+            x.run.status[s.begin + i] = j.status;
+        }
         if (!s.host_decoded[i]) {
             if (sc.status == 0 && sc.nrows >= 2) {
                 j.padbit = (int8_t)sc.padbit;
@@ -457,8 +472,10 @@ void select_segments(CompressCall& x, ChunkState& s) {
             x.run.status[s.begin + i] = j.status;
         }
         fill_image(s.imgs[q], j, s.planes[i].data(), s.splits[i].selected);
-        if (!s.host_decoded[i] && j.status == 0) {
-            // decision-count bound of each thread-segment from the per-row counters of the Huffman kernel
+        // decision-count bound of each thread-segment from the per-row counters of the Huffman kernel.  A scan whose data
+        // ends before its last MCU row leaves blocks that no row counted and that the encoder still codes: such an image
+        // keeps the bound 0, and the library counts its decisions itself.
+        if (!s.host_decoded[i] && j.status == 0 && sc.rows[sc.nrows - 1].mcu_y >= j.mcuv) {
             lepb200_image& im = s.imgs[q];
             size_t r = 0;
             uint32_t start_tok[LEPB200_MAX_SEGMENTS + 1];
@@ -530,7 +547,7 @@ void compress_back(CompressCall& x, int k) {
         });
     }
     parallel_for((int)s.js.size(), bth, [&](int i) { s.js[i].reset(); });     // release per-chunk host state early
-    s.js.clear(); s.planes.clear(); s.splits.clear();
+    s.js.clear(); s.planes.clear(); s.splits.clear(); s.redo_planes.clear();
     x.run.mark("back", k, t0);
     x.run.add_time(0, 0, now_s() - t0);
 }
@@ -1153,6 +1170,7 @@ int lepb200_decompress_leps_multi(lepb200_codec* const* codecs, int ncodecs, con
 // thread-segment split as a lepb200_image, and assemble the .lep from externally coded segment streams.
 struct lepb200_jpeg {
     Jpeg j;
+    bool parsed = false;             // the headers and the scan were read (the Huffman decode may still have failed)
     Splits sp;
     std::vector<std::vector<int16_t>> store;
     int16_t* planes[4] = {nullptr, nullptr, nullptr, nullptr};
@@ -1176,7 +1194,8 @@ int lepb200_host_jpeg_open_embedded(const uint8_t* data, size_t len, int min_thr
     if (!out || !data) return LEPB200_ERR_INVALID;
     lepb200_jpeg* h = new lepb200_jpeg();
     *out = h;
-    if (parse_jpeg(data, len, h->j, embedding < 0 ? -1 : embedding, discard_meta != 0)) {
+    h->parsed = parse_jpeg(data, len, h->j, embedding < 0 ? -1 : embedding, discard_meta != 0);
+    if (h->parsed) {
         h->store.resize(h->j.ncmp);
         for (int c = 0; c < h->j.ncmp; ++c) {
             h->store[c].assign((size_t)h->j.cmp[c].bc * 64, 0);
@@ -1197,7 +1216,7 @@ int lepb200_host_jpeg_image(lepb200_jpeg* h, lepb200_image* img) {
 }
 
 int lepb200_host_jpeg_scan(lepb200_jpeg* h, lepb200_jpeg_scan* sc) {
-    if (!h || !sc || h->j.status) return LEPB200_ERR_INVALID;
+    if (!h || !sc || !h->parsed) return LEPB200_ERR_INVALID;
     const Jpeg& j = h->j;
     GpuScanSetup gs;
     if (!gpu_scan_setup(j, gs)) return LEPB200_ERR_INVALID;

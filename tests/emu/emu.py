@@ -167,8 +167,8 @@ def huffman_decode(mode, jpegs, sub_bits=4096, iter_cap=62, mutate=None, reverse
     """Huffman-decodes whole JPEG files with the emulated kernels.  mode HUFF_SERIAL: lep_huffdecode_kernel (one warp per
     image); HUFF_SUBSEQ: the sub-sequence kernels of lep_huffpar.cu, then lep_huffdecode_kernel for what they left.
     Returns (results, info): per file None when the host front end does not hand the file to the GPU decoder, else a dict
-    with status, padbit, end_bitpos, rows [(bitpos, lastdc, mcu_y, tokens)], planes [ndarray(blocks, 64)], host_planes,
-    and the scan's nbytes (de-stuffed), ncmp and rsti;
+    with status, padbit, end_bitpos, rows [(bitpos, lastdc, mcu_y, tokens)], planes [ndarray(blocks, 64)], host_status,
+    host_planes (None where the host decoder refused the scan), and the scan's nbytes (de-stuffed), ncmp and rsti;
     info = (synchronisation iterations, images the serial kernel had to redo).  `mutate(i, bytearray)` may damage the
     de-stuffed entropy bytes of file i before decoding.  reverse runs the CTAs and threads of every launch in reverse order."""
     from lepton_b200.codec import HostJpeg, lib as product_lib
@@ -180,7 +180,7 @@ def huffman_decode(mode, jpegs, sub_bits=4096, iter_cap=62, mutate=None, reverse
         hj = HostJpeg(data)
         hjs.append(hj)
         sc = _Scan()
-        if hj.status != 0 or L.lepb200_host_jpeg_scan(hj._h, ctypes.byref(sc)) != 0:
+        if L.lepb200_host_jpeg_scan(hj._h, ctypes.byref(sc)) != 0:
             continue
         if mutate is not None:
             buf = bytearray(ctypes.string_at(sc.entropy, sc.nbytes))
@@ -216,8 +216,9 @@ def huffman_decode(mode, jpegs, sub_bits=4096, iter_cap=62, mutate=None, reverse
     for k, i in enumerate(idx):
         sc = arr[k]
         rows = [(sc.rows[r].bitpos, tuple(sc.rows[r].lastdc), sc.rows[r].mcu_y, sc.rows[r].tokens) for r in range(max(0, min(sc.nrows, sc.mcuv + 1)))]
-        host = [np.array(p) for p in hjs[i].coef_image().planes] if mutate is None else None
-        res[i] = dict(status=sc.status, padbit=sc.padbit, end_bitpos=sc.end_bitpos, nrows=sc.nrows, rows=rows, planes=planes[k], host_planes=host,
+        host = [np.array(p) for p in hjs[i].coef_image().planes] if mutate is None and hjs[i].status == 0 else None
+        res[i] = dict(status=sc.status, padbit=sc.padbit, end_bitpos=sc.end_bitpos, nrows=sc.nrows, rows=rows, planes=planes[k],
+                      host_status=hjs[i].status, host_planes=host,
                       nbytes=sc.nbytes, ncmp=sc.ncmp, rsti=sc.rsti)
     return res, (info[0], info[1])
 

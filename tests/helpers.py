@@ -65,6 +65,33 @@ def load_dense_lep(name):
     return lepfmt.parse_container(read_golden("dense/" + name))
 
 
+# complete JPEGs (EOI present) with short, damaged or oddly padded scans and what the reference CLI made of them
+# (tests/golden/make_shortscan.py)
+SHORTSCAN = json.load(open(os.path.join(GOLDEN, "shortscan.json")))
+
+
+def shortscan_jpegs():
+    return sorted(SHORTSCAN)
+
+
+# Files of that corpus that the library refuses with UNSUPPORTED_JPEG (42) although the reference run with -skipverify
+# writes a .lep: the data runs out inside a block whose Huffman code is then invalid, and the reference's scan loop ends
+# the scan at eof whatever its block decoder returned, dropping that block.  Its .lep does not restore the input (the
+# reference's own verifying run refuses the file with ROUNDTRIP_FAILURE, 41), so the library keeps the refusal rather
+# than write a container that loses the file.
+SHORTSCAN_REFUSED = {"c420_cut_row.jpg": 42}
+
+
+def shortscan_status(name):
+    """The status the library reports for a file of the short-scan corpus."""
+    return SHORTSCAN_REFUSED.get(name, SHORTSCAN[name]["status_want"])
+
+
+def shortscan_lep(name):
+    """The reference's .lep of an accepted short-scan file."""
+    return read_golden("shortscan/" + name[:-4] + ".lep")
+
+
 # small baseline JPEGs cut at every byte of their scan and what the reference CLI made of every cut
 # (tests/golden/make_truncated.py)
 TRUNCATED = json.load(open(os.path.join(GOLDEN, "truncated.json")))

@@ -41,10 +41,10 @@ class BitWriter:
             self.n -= 8
         self.acc &= (1 << self.n) - 1
 
-    def pad(self):
-        """Fill the last byte with 1 bits (what libjpeg and the reference expect before a marker)."""
+    def pad(self, bit=1):
+        """Fill the last byte with `bit` (1 is what libjpeg and the reference expect before a marker)."""
         while self.n & 7:
-            self.put(1, 1)
+            self.put(bit, 1)
 
 
 def canonical_codes(bits, vals):
@@ -146,10 +146,11 @@ def geometry(width, height, sampling):
 
 
 def write_baseline(planes, width, height, sampling, qtables, qbits=8, dc_tables=None, ac_tables=None, restart=0,
-                   extra_markers=b""):
+                   extra_markers=b"", padbit=1):
     """planes[c]: int array (mcuv * V, mcuh * H, 64), zig-zag order.  qtables: one 64-entry table (zig-zag order) per
     component or one for all; dc_tables / ac_tables: HuffTable for luma and for chroma (one table serves all components when
-    only one is given).  restart: DRI interval in MCUs (0 = none).  Returns the file bytes."""
+    only one is given).  restart: DRI interval in MCUs (0 = none).  padbit: the bit that fills the last byte of every
+    restart interval, or a list of them, one per interval.  Returns the file bytes."""
     ncmp = len(planes)
     assert ncmp in (1, 3) and len(sampling) == ncmp
     dc_tables = dc_tables or [uniform_table(DC_SYMBOLS[:12], 5)]
@@ -185,14 +186,15 @@ def write_baseline(planes, width, height, sampling, qtables, qbits=8, dc_tables=
                  for my in range(mcuv) for mx in range(mcuh)]
     bw = BitWriter()
     pred = [0] * ncmp
+    pads = [padbit] * (len(units) + 1) if isinstance(padbit, int) else list(padbit)
     for i, unit in enumerate(units):
         if restart and i and i % restart == 0:
-            bw.pad()
+            bw.pad(pads[i // restart - 1])
             bw.out += bytes([0xFF, 0xD0 + ((i // restart - 1) & 7)])
             pred = [0] * ncmp
         for c, by, bx in unit:
             pred[c] = put_block(bw, planes[c][by, bx], pred[c], dc_tables[tidx[c]].enc, ac_tables[aidx[c]].enc)
-    bw.pad()
+    bw.pad(pads[(len(units) - 1) // restart if restart else 0])
     o += bw.out + b"\xff\xd9"
     return bytes(o)
 

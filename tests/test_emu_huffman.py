@@ -73,8 +73,13 @@ def test_synthetic_jpegs_subsequence_kernels(w, h, q, sub):
 
 def test_damaged_scans_fall_back_to_the_serial_walk():
     """Bit flips, a cut-off tail and appended junk: whatever the sub-sequence kernels meet, the outcome (status and, for
-    status 0, every output) is the serial kernel's, under both schedules."""
-    jpegs = [pil_jpeg(100 + k, 320, 240) for k in range(6)]
+    status 0, every output) is the serial kernel's, under both schedules.  The short-scan corpus rides along untouched
+    (complete files whose scan is short, damaged or oddly padded, tests/golden/make_shortscan.py): the serial kernel's
+    status is the host decoder's, or "not handled" (200) where the data ends inside a block or a zero run passes the end
+    of one -- the file API gives those to the host decoder."""
+    from helpers import SHORTSCAN, shortscan_jpegs
+    short = [n for n in shortscan_jpegs() if SHORTSCAN[n]["path"].startswith("shortscan/")]
+    jpegs = [pil_jpeg(100 + k, 320, 240) for k in range(6)] + [open(os.path.join(GOLDEN, SHORTSCAN[n]["path"]), "rb").read() for n in short]
 
     def mutate(i, buf):
         if i == 1:
@@ -90,7 +95,10 @@ def test_damaged_scans_fall_back_to_the_serial_walk():
             buf[-1] ^= 0x01
     ser, _ = emu.huffman_decode(emu.HUFF_SERIAL, jpegs, mutate=mutate)
     assert ser[0]["status"] == 0
-    assert any(s["status"] != 0 for s in ser[1:])
+    assert any(s["status"] != 0 for s in ser[1:6])
+    for n, s in zip(short, ser[6:]):
+        assert s["status"] in (s["host_status"], 200), (n, s["status"], s["host_status"])
+    assert {s["status"] for s in ser[6:]} == {0, 42, 200}
     for reverse in (False, True):
         par, (iters, redo) = emu.huffman_decode(emu.HUFF_SUBSEQ, jpegs, sub_bits=1024, mutate=mutate, reverse=reverse)
         for k, (s, p) in enumerate(zip(ser, par)):

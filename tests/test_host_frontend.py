@@ -9,7 +9,8 @@ import numpy as np
 import pytest
 
 import lepfmt
-from helpers import EXTREMES, GOLDEN, MANIFEST, extreme_leps, load_extreme_lep, load_lep, plane_hashes, read_golden
+from helpers import (EXTREMES, GOLDEN, MANIFEST, SHORTSCAN, SHORTSCAN_REFUSED, extreme_leps, load_extreme_lep, load_lep, plane_hashes,
+                     read_golden, shortscan_jpegs, shortscan_lep)
 
 BASELINE_COMPLETE = ["android.jpg", "androidcrop.jpg", "androidcropoptions.jpg", "androidtrail.jpg", "colorswap.jpg",
                      "grayscale.jpg", "iphonecrop2.jpg", "trailingrst.jpg", "trailingrst2.jpg"]
@@ -17,11 +18,37 @@ BASELINE_COMPLETE = ["android.jpg", "androidcrop.jpg", "androidcropoptions.jpg",
 BASELINE_TRUNCATED = ["gray2sf.jpg", "narrowrst.jpg", "nofsync.jpg", "singlerowtrunc.jpg", "truncatedzerorun.jpg"]
 # progressive (spectral selection + successive approximation, end-of-band runs, correction bits): container flag 'X'
 PROGRESSIVE = ["androidprogressive.jpg", "iphoneprogressive.jpg", "iphoneprogressive2.jpg"]
+# complete files with short, damaged or oddly padded scans (tests/golden/make_shortscan.py)
+SHORTSCAN_CASES = [n for n in shortscan_jpegs() if n != "badzerorun.jpg"]
 
 
-@pytest.mark.parametrize("name", BASELINE_COMPLETE + BASELINE_TRUNCATED + PROGRESSIVE)
+def check_shortscan(name):
+    """Host status as the reference's (6 is the coder's refusal: the front end takes the file), or the refusal the
+    library keeps where the reference writes a .lep that does not restore the file; for accepted files the oracle's
+    streams over the host planes are the reference's, and the container built around them is its file."""
+    from lepton_b200 import HostJpeg
+    from helpers import oracle_encode_image, shortscan_status
+    e = SHORTSCAN[name]
+    want = shortscan_status(name)
+    if name in SHORTSCAN_REFUSED:
+        assert e["rc_verify"] == 41 and e["back_md5"] != e["jpg_md5"], "the reference's .lep of this file restores it"
+    hj = HostJpeg(read_golden(e["path"]))
+    assert hj.status == (0 if want == 6 else want), (hj.status, hj.error)
+    if want != 0:
+        return
+    ref = shortscan_lep(name)
+    lf = lepfmt.parse_container(ref)
+    streams = lepfmt.demux(lf.payload)[:lf.nseg]
+    img = hj.coef_image()
+    assert [s for _, s, _ in oracle_encode_image(img)] == streams, "host planes differ from the reference's"
+    assert hj.write_lep(streams) == ref
+
+
+@pytest.mark.parametrize("name", BASELINE_COMPLETE + BASELINE_TRUNCATED + PROGRESSIVE + SHORTSCAN_CASES)
 def test_jpeg_front_end_and_container_match_reference(name):
     from lepton_b200 import HostJpeg
+    if name in SHORTSCAN:
+        return check_shortscan(name)
     data = open(os.path.join(GOLDEN, name), "rb").read()
     hj = HostJpeg(data)
     assert hj.status == 0, hj.error
