@@ -119,6 +119,12 @@ int lepb200_encode_upload_tokens(lepb200_ctx* ctx, const uint16_t* tokens, const
 /* After the fetch of such a batch: moved[s] = 1 where stream s was placed in the overflow arena (it did not fit its slot),
  * *changed = canary bytes overwritten behind the slots and behind the streams of the overflow arena. */
 int lepb200_encode_token_canaries(lepb200_ctx* ctx, uint8_t* moved, uint64_t* changed);
+/* lepb200_encode_upload_tokens with the entropy coder of every segment: coders[s] (LEPB200_CODER_*) for segment s, NULL = all
+ * LEPB200_CODER_BOOL (then exactly lepb200_encode_upload_tokens).  lepb200_encode_launch_rangecode codes the rANS segments
+ * with the rANS pass: their streams are written into their token slots, so caps[s] does not matter for them and
+ * lepb200_encode_token_canaries reports them as moved.  Fetch with lepb200_encode_fetch. */
+int lepb200_encode_upload_tokens_coded(lepb200_ctx* ctx, const uint16_t* tokens, const uint32_t* ntok, const uint32_t* caps, int nseg,
+                                       const int32_t* seg_per_file, int nfiles, const uint8_t* coders);
 int lepb200_decode_upload(lepb200_ctx* ctx, const lepb200_image* images, int nimages, const lepb200_stream* in);
 int lepb200_decode_launch(lepb200_ctx* ctx);
 int lepb200_decode_fetch(lepb200_ctx* ctx, const lepb200_image* images, int nimages, int32_t* status_out);
@@ -264,6 +270,13 @@ int lepb200_decode_upload_gather(lepb200_ctx* ctx, const lepb200_image* images, 
  * update of the branch counts (Branch::adv_record_obs_and_update) and other bits. */
 #define LEPB200_CODER_BOOL 0
 #define LEPB200_CODER_ANS 1
+/* lepb200_encode_upload / lepb200_encode_images with the coder of every image: coders[i] (LEPB200_CODER_*) for image i,
+ * NULL = all LEPB200_CODER_BOOL (then exactly the forms without it).  A batch may mix coders: kernel A runs once per coder,
+ * the bool coder's range coder codes the bool-coded segments and the rANS pass the rANS-coded ones (container version 3,
+ * the reference's -ans).  The streams come back through lepb200_encode_fetch in the caller's order;
+ * lepb200_encode_fetch_files refuses a batch with rANS-coded segments (LEPB200_ERR_INVALID): it writes version-1 files only. */
+int lepb200_encode_upload_coded(lepb200_ctx* ctx, const lepb200_image* images, int nimages, const uint8_t* coders);
+int lepb200_encode_images_coded(lepb200_ctx* ctx, const lepb200_image* images, int nimages, const uint8_t* coders, lepb200_stream* out);
 /* lepb200_decode_upload / lepb200_decode_upload_gather with the coder of every image: coders[i] (LEPB200_CODER_*) for image i,
  * NULL = all LEPB200_CODER_BOOL (then exactly the forms without it).  A batch may mix coders: the segments of each coder are
  * decoded by launches of their own, each choosing its kernel by its own size.  Launch and fetch as for the plain forms. */

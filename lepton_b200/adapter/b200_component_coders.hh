@@ -78,7 +78,13 @@ public:
         im.nseg = (int32_t)num_selected_splits;
         for (unsigned i = 0; i < num_selected_splits; ++i) im.luma_y_start[i] = selected_splits[i].luma_y_start;
         lepb200_stream s[LEPB200_MAX_SEGMENTS];
+#ifdef ENABLE_ANS_EXPERIMENTAL
+        // -ans (container version 3, jpgcoder.cc:1704-1705): rANS-coded segment streams
+        const uint8_t coder = ujgversion == 3 ? LEPB200_CODER_ANS : LEPB200_CODER_BOOL;
+        lepb200_adapter::exit_on(lepb200_encode_images_coded(ctx_, &im, 1, &coder, s));
+#else
         lepb200_adapter::exit_on(lepb200_encode_images(ctx_, &im, 1, s));
+#endif
         for (unsigned i = 0; i < num_selected_splits; ++i) {
             if (s[i].status) custom_exit((ExitCode)s[i].status);   // the reference's own ExitCode values
         }
@@ -134,7 +140,16 @@ class B200ComponentDecoder : public BaseDecoder {
             s[i].len = (uint64_t)(seg[i].second - seg[i].first);
         }
         int32_t st[LEPB200_MAX_SEGMENTS];
+#ifdef ENABLE_ANS_EXPERIMENTAL
+        // a version-3 file's streams are rANS-coded (the reference's makeDecoder(..., ujgversion == 3), jpgcoder.cc:1727);
+        // every decoder entry (decode_chunk, the row entry, -singlethread) comes through here
+        const uint8_t coder = ujgversion == 3 ? LEPB200_CODER_ANS : LEPB200_CODER_BOOL;
+        lepb200_adapter::exit_on(lepb200_decode_upload_coded(ctx_, &im, 1, s, &coder));
+        lepb200_adapter::exit_on(lepb200_decode_launch(ctx_));
+        lepb200_adapter::exit_on(lepb200_decode_fetch(ctx_, &im, 1, st));
+#else
         lepb200_adapter::exit_on(lepb200_decode_images(ctx_, &im, 1, s, st));
+#endif
         for (int i = 0; i < nseg; ++i) {
             if (st[i]) custom_exit((ExitCode)st[i]);
         }
@@ -228,7 +243,8 @@ public:
     void reset_all_comm_buffers() {}
 };
 
-// The two lines that change in the reference (src/lepton/jpgcoder.cc):
+// The lines that change in the reference (src/lepton/jpgcoder.cc; with -DENABLE_ANS_EXPERIMENTAL also :1705, the rANS
+// encoder's  g_encoder.reset(makeEncoder<ANSBoolReader>(g_threaded, g_threaded));  ->  g_encoder.reset(new B200ComponentEncoder);):
 //   :1710   g_encoder.reset(makeEncoder<VPXBoolReader>(g_threaded, g_threaded));   ->  g_encoder.reset(new B200ComponentEncoder);
 //   :1727   g_decoder = makeDecoder(g_threaded, g_threaded, ujgversion == 3);       ->  g_decoder = new B200ComponentDecoder;
 //           followed, as in makeBoth (:440-452), by  if (g_threaded) g_decoder->registerWorkers(get_worker_threads(NUM_THREADS), NUM_THREADS);

@@ -69,6 +69,7 @@ _EXPORTS = [
     "lepb200_codec_set_permissive", "lepb200_host_generic_lep", "lepb200_host_lep_generic",
     "lepb200_decode_upload_coded", "lepb200_decode_upload_gather_coded", "lepb200_host_lep_coder",
     "lepb200_decode_fetch_decisions",
+    "lepb200_encode_upload_coded", "lepb200_encode_images_coded", "lepb200_encode_upload_tokens_coded",
 ]
 
 CODER_BOOL, CODER_ANS = 0, 1          # LEPB200_CODER_*: bool coder (container versions 1, 2, 4), rANS coder (version 3)
@@ -103,6 +104,12 @@ def lib():
     L.lepb200_encode_upload.argtypes = [vp, ip, ctypes.c_int]
     L.lepb200_encode_launch.argtypes = [vp]
     L.lepb200_encode_fetch.argtypes = [vp, sp]
+    L.lepb200_encode_upload_coded.argtypes = [vp, ip, ctypes.c_int, ctypes.POINTER(ctypes.c_uint8)]
+    L.lepb200_encode_upload_coded.restype = ctypes.c_int
+    L.lepb200_encode_images_coded.argtypes = [vp, ip, ctypes.c_int, ctypes.POINTER(ctypes.c_uint8), sp]
+    L.lepb200_encode_images_coded.restype = ctypes.c_int
+    L.lepb200_encode_upload_tokens_coded.argtypes = [vp, vp, vp, vp, ctypes.c_int, vp, ctypes.c_int, ctypes.POINTER(ctypes.c_uint8)]
+    L.lepb200_encode_upload_tokens_coded.restype = ctypes.c_int
     L.lepb200_decode_images.argtypes = [vp, ip, ctypes.c_int, sp, ctypes.POINTER(ctypes.c_int32)]
     L.lepb200_decode_upload.argtypes = [vp, ip, ctypes.c_int, sp]
     L.lepb200_decode_upload_coded.argtypes = [vp, ip, ctypes.c_int, sp, ctypes.POINTER(ctypes.c_uint8)]
@@ -214,10 +221,18 @@ class LeptonB200Codec:
             arr[i] = im.to_c()
         return arr
 
-    def encode_upload(self, images):
+    def encode_upload(self, images, coders=None):
+        """coders: per image, the entropy coder of its segment streams (CODER_BOOL, or CODER_ANS for the rANS streams of
+        container version 3); None = all CODER_BOOL."""
         self._enc_imgs = images
         self._enc_c = self._c_images(images)
-        self._check(self._L.lepb200_encode_upload(self._ctx, self._enc_c, len(images)), "encode_upload")
+        if coders is None:
+            self._check(self._L.lepb200_encode_upload(self._ctx, self._enc_c, len(images)), "encode_upload")
+        else:
+            if len(coders) != len(images):
+                raise LeptonB200Error("one coder per image")
+            cod = (ctypes.c_uint8 * len(images))(*[int(c) for c in coders])
+            self._check(self._L.lepb200_encode_upload_coded(self._ctx, self._enc_c, len(images), cod), "encode_upload")
 
     def encode_launch(self):
         self._check(self._L.lepb200_encode_launch(self._ctx), "encode_launch")
@@ -238,8 +253,9 @@ class LeptonB200Codec:
         self.last_lens = [out[i].len for i in range(n)]
         return res
 
-    def encode_images(self, images, copy=True):
-        self.encode_upload(images)
+    def encode_images(self, images, copy=True, coders=None):
+        """Per image, a list of SegmentResult per segment.  coders: as for encode_upload."""
+        self.encode_upload(images, coders)
         self.encode_launch()
         return self.encode_fetch(copy=copy)
 
@@ -308,9 +324,11 @@ class LeptonB200Codec:
         self.decode_launch()
         return self.decode_fetch()
 
-    def range_code(self, streams, caps, files=None, headers=None):
+    def range_code(self, streams, caps, files=None, headers=None, coders=None):
         """The range coder alone, on caller token streams (lepb200_encode_upload_tokens), launched and fetched as an encode
-        batch is: streams = uint16 token arrays (prob | bit << 8), caps = stream slot of each in bytes.
+        batch is: streams = uint16 token arrays (prob | bit << 8), caps = stream slot of each in bytes.  coders: per
+        segment, CODER_BOOL or CODER_ANS (the rANS pass; such a stream is written into its token slot and reports moved);
+        None = all CODER_BOOL.
         Without headers -> (per segment (status, bytes, moved to the overflow arena), changed canary bytes).
         With files (segments per file, consecutive) and headers (per file everything in front of the mux packets) the
         files are assembled on the device (lepb200_encode_fetch_files) -> (per file (status, bytes), moved, changed)."""
@@ -326,7 +344,13 @@ class LeptonB200Codec:
                                                    ctypes.c_void_p, ctypes.c_int]
         L.lepb200_encode_launch_rangecode.argtypes = [ctypes.c_void_p]
         L.lepb200_encode_token_canaries.argtypes = [ctypes.c_void_p, ctypes.c_void_p, ctypes.POINTER(ctypes.c_uint64)]
-        self._check(L.lepb200_encode_upload_tokens(self._ctx, flat.ctypes.data, nt, cp, n, spf, len(files)), "encode_upload_tokens")
+        if coders is None:
+            self._check(L.lepb200_encode_upload_tokens(self._ctx, flat.ctypes.data, nt, cp, n, spf, len(files)), "encode_upload_tokens")
+        else:
+            if len(coders) != n:
+                raise LeptonB200Error("one coder per segment")
+            cod = (ctypes.c_uint8 * n)(*[int(c) for c in coders])
+            self._check(L.lepb200_encode_upload_tokens_coded(self._ctx, flat.ctypes.data, nt, cp, n, spf, len(files), cod), "encode_upload_tokens")
         self._check(L.lepb200_encode_launch_rangecode(self._ctx), "encode_launch_rangecode")
         if headers is None:
             out = (_Stream * n)()

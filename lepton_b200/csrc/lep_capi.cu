@@ -216,11 +216,11 @@ int build_batch(lepb200_ctx* ctx, const lepb200_image* images, int nimages, bool
     BatchPlan& b = ctx->batch;
     if (const char* e = plan_batch(b, images, nimages, encode, in, coders)) { ctx->err = e; return LEPB200_ERR_INVALID; }
     const int nseg = (int)b.segs.size();
-    const int nbool = encode ? nseg : b.order_ans;      // decode: the bool-coded segments, launched before the rANS-coded ones
+    const int nbool = b.order_ans;                      // the bool-coded segments, launched before the rANS-coded ones
 
     // persistent grid: as many CTAs as can be resident, but no more warps than segments
     int per_sm = 0;
-    if (encode) CK(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, lep_encode_kernel, ENC_WARPS_PER_CTA * 32, 0));
+    if (encode) CK(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, lep_encode_kernel<EncBool>, ENC_WARPS_PER_CTA * 32, 0));
     else CK(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, lep_decode_kernel<BoolReader>, DEC_WARPS_PER_CTA * 32, 0));
     if (encode && ctx->enc_cta_cap > 0) per_sm = std::min(per_sm, ctx->enc_cta_cap);
     const int wpc = encode ? ENC_WARPS_PER_CTA : DEC_WARPS_PER_CTA;
@@ -265,6 +265,21 @@ int build_batch(lepb200_ctx* ctx, const lepb200_image* images, int nimages, bool
     CK(cudaMemcpyAsync(ctx->d_segs.p, b.segs.data(), sizeof(SegDesc) * nseg, cudaMemcpyHostToDevice, ctx->stream));
     CK(cudaMemcpyAsync(ctx->d_order.p, b.order.data(), sizeof(int) * nseg, cudaMemcpyHostToDevice, ctx->stream));
     return 0;
+}
+
+// lep_compact_kernel for batches with rANS-coded segments: their streams lie in the token arena, 4-byte aligned (the rANS
+// pass writes them backward from the end of the token slot), so the body moves 4-byte words
+__global__ void lep_compact4_kernel(const SegDesc* __restrict__ segs, const unsigned long long* __restrict__ dst_off, uint8_t* __restrict__ dense, int nseg) {
+    const int s = blockIdx.x;
+    if (s >= nseg) return;
+    const uint8_t* src = reinterpret_cast<const uint8_t*>(segs[s].stream);
+    uint8_t* dst = dense + dst_off[s];
+    const uint32_t n = segs[s].status == 0 ? segs[s].len : 0;
+    const uint32_t n4 = n / 4;
+    const uint32_t* s4 = reinterpret_cast<const uint32_t*>(src);
+    uint32_t* d4 = reinterpret_cast<uint32_t*>(dst);
+    for (uint32_t i = threadIdx.x; i < n4; i += blockDim.x) d4[i] = s4[i];
+    for (uint32_t i = n4 * 4 + threadIdx.x; i < n; i += blockDim.x) dst[i] = src[i];
 }
 
 __global__ void lep_compact_kernel(const SegDesc* __restrict__ segs, const unsigned long long* __restrict__ dst_off, uint8_t* __restrict__ dense, int nseg) {
@@ -410,9 +425,13 @@ void lepb200_pinned_free(void* p) { if (p) cudaFreeHost(p); }
 
 // ------------------------------------------------------------------------------------------------ encode
 int lepb200_encode_upload(lepb200_ctx* ctx, const lepb200_image* images, int nimages) {
+    return lepb200_encode_upload_coded(ctx, images, nimages, nullptr);
+}
+
+int lepb200_encode_upload_coded(lepb200_ctx* ctx, const lepb200_image* images, int nimages, const uint8_t* coders) {
     if (!ctx) return LEPB200_ERR_INVALID;
     CK(cudaSetDevice(ctx->device));
-    int r = build_batch(ctx, images, nimages, true, nullptr);
+    int r = build_batch(ctx, images, nimages, true, nullptr, coders);
     if (r) return r;
     for (int i = 0; i < nimages; ++i)
         for (int c = 0; c < images[i].ncmp; ++c)
@@ -619,16 +638,30 @@ int lepb200_encode_upload_resident(lepb200_ctx* ctx, const lepb200_image* images
 int lepb200_encode_launch_symbolise(lepb200_ctx* ctx) {
     if (!ctx || !ctx->have_batch || !ctx->is_encode) { if (ctx) ctx->err = "encode_launch without encode_upload"; return LEPB200_ERR_INVALID; }
     CK(cudaSetDevice(ctx->device));
-    const int nseg = (int)ctx->batch.segs.size();
-    CK(cudaMemsetAsync(ctx->d_counter.p, 0, sizeof(int), ctx->stream));
+    const int nseg = (int)ctx->batch.segs.size(), nbool = ctx->batch.order_ans;
+    // one launch per coder: the bool-coded segments (order[0 .. nbool)), then the rANS-coded ones, each with its own queue
+    // (the rANS part's work counter sits 32 bytes into the counter buffer)
+    int* dcnt = static_cast<int*>(ctx->d_counter.p);
+    CK(cudaMemsetAsync(ctx->d_counter.p, 0, nbool < nseg ? 64 : sizeof(int), ctx->stream));
     CK(cudaEventRecord(ctx->ev0, ctx->stream));
-    lep_encode_kernel<<<ctx->grid, ENC_WARPS_PER_CTA * 32, 0, ctx->stream>>>(
-        static_cast<const ImageDesc*>(ctx->d_images.p), static_cast<SegDesc*>(ctx->d_segs.p), nseg, static_cast<const int*>(ctx->d_order.p),
-        static_cast<int*>(ctx->d_counter.p), static_cast<uint16_t*>(ctx->d_models.p), static_cast<uint8_t*>(ctx->d_rows.p), ctx->batch.row_stride,
-        static_cast<uint16_t*>(ctx->d_tokens.p));
-    CK(cudaGetLastError());
+    const ImageDesc* di = static_cast<const ImageDesc*>(ctx->d_images.p);
+    SegDesc* ds = static_cast<SegDesc*>(ctx->d_segs.p);
+    const int* dord = static_cast<const int*>(ctx->d_order.p);
+    uint16_t* dm = static_cast<uint16_t*>(ctx->d_models.p);
+    uint8_t* dr = static_cast<uint8_t*>(ctx->d_rows.p);
+    uint16_t* dt = static_cast<uint16_t*>(ctx->d_tokens.p);
+    if (nbool > 0) {
+        lep_encode_kernel<EncBool><<<ctx->grid, ENC_WARPS_PER_CTA * 32, 0, ctx->stream>>>(di, ds, nbool, dord, dcnt, dm, dr, ctx->batch.row_stride, dt);
+        CK(cudaGetLastError());
+        ctx->launches += 1;
+    }
+    if (nbool < nseg) {
+        lep_encode_kernel<EncAns><<<ctx->grid_ans, ENC_WARPS_PER_CTA * 32, 0, ctx->stream>>>(di, ds, nseg - nbool, dord + nbool, dcnt + 8, dm, dr,
+                                                                                               ctx->batch.row_stride, dt);
+        CK(cudaGetLastError());
+        ctx->launches += 1;
+    }
     CK(cudaEventRecord(ctx->ev_mid, ctx->stream));
-    ctx->launches += 1;
     ctx->symbolised = true;
     return LEPB200_OK;
 }
@@ -636,9 +669,13 @@ int lepb200_encode_launch_symbolise(lepb200_ctx* ctx) {
 int lepb200_encode_launch_rangecode(lepb200_ctx* ctx) {
     if (!ctx || !ctx->symbolised || !ctx->is_encode) { if (ctx) ctx->err = "encode_launch_rangecode without encode_launch_symbolise"; return LEPB200_ERR_INVALID; }
     CK(cudaSetDevice(ctx->device));
-    const int nseg = (int)ctx->batch.segs.size();
+    // the bool-coded segments are segs[0 .. nbool) and order[0 .. nbool) (plan_batch): the range coder takes those, the
+    // rANS pass the others, in every rc_mode
+    const int nall = (int)ctx->batch.segs.size(), nseg = ctx->batch.order_ans;
     ctx->rc_ovf_used = 0;
-    if (ctx->rc_mode == 1) {
+    if (nseg == 0) {
+        // no bool-coded segment
+    } else if (ctx->rc_mode == 1) {
         // range-only pass -> digit layout (one small D2H + sync: the arena size depends on the data) -> parallel pieces -> carries
         SegDesc* ds = static_cast<SegDesc*>(ctx->d_segs.p);
         const int* dord = static_cast<const int*>(ctx->d_order.p);
@@ -679,14 +716,22 @@ int lepb200_encode_launch_rangecode(lepb200_ctx* ctx) {
             fprintf(stderr, "[trace]   range coder: range pass + offsets %.1f ms, pieces (incl. digit zero fill) %.1f ms, carries %.1f ms, %d segments\n", a, b, c, nseg);
             for (auto& e : te) cudaEventDestroy(e);
         }
-        ctx->launches += 3;
+        ctx->launches += 4;
     } else {
         lep_rangecode_kernel<<<(nseg + RC_THREADS - 1) / RC_THREADS, RC_THREADS, 0, ctx->stream>>>(
             static_cast<SegDesc*>(ctx->d_segs.p), nseg, static_cast<const int*>(ctx->d_order.p), static_cast<const uint16_t*>(ctx->d_tokens.p));
         CK(cudaGetLastError());
+        ctx->launches += 1;
+    }
+    if (nall > nseg) {
+        // rANS pass (lep_encode.cu): one thread per segment, the stream written in place into the segment's token slot
+        const int n = nall - nseg;
+        lep_anspass_kernel<<<(n + ANS_THREADS - 1) / ANS_THREADS, ANS_THREADS, 0, ctx->stream>>>(
+            static_cast<SegDesc*>(ctx->d_segs.p), n, static_cast<const int*>(ctx->d_order.p) + nseg, static_cast<uint16_t*>(ctx->d_tokens.p));
+        CK(cudaGetLastError());
+        ctx->launches += 1;
     }
     CK(cudaEventRecord(ctx->ev1, ctx->stream));
-    ctx->launches += 1;
     ctx->symbolised = false;
     ctx->launched = true;
     return LEPB200_OK;
@@ -702,7 +747,7 @@ int lepb200_encode_launch(lepb200_ctx* ctx) {
 static int rerun_overflowed_serial(lepb200_ctx* ctx, SegDesc* hs, int nseg) {
     if (ctx->rc_mode == 1) return LEPB200_OK;
     std::vector<int>& redo = ctx->rc_redo;
-    const size_t total = plan_serial_rerun(hs, nseg, redo);
+    const size_t total = plan_serial_rerun(hs, ctx->batch.order_ans, redo);       // the bool-coded segments, segs[0 .. order_ans)
     if (redo.empty()) return LEPB200_OK;
     CK(reserve_overflow(ctx, total));
     CK(ctx->d_rc_redo.reserve(sizeof(int) * redo.size()));
@@ -745,17 +790,22 @@ int lepb200_encode_fetch(lepb200_ctx* ctx, lepb200_stream* out) {
     CK(ctx->h_dense.reserve(total + 16));
     unsigned long long* d_offs = reinterpret_cast<unsigned long long*>(static_cast<uint8_t*>(ctx->d_dense.p) + dense_bytes);
     CK(cudaMemcpyAsync(d_offs, offs, sizeof(unsigned long long) * nseg, cudaMemcpyHostToDevice, ctx->stream));
-    lep_compact_kernel<<<nseg, 256, 0, ctx->stream>>>(static_cast<const SegDesc*>(ctx->d_segs.p), d_offs, static_cast<uint8_t*>(ctx->d_dense.p), nseg);
+    if (ctx->batch.order_ans == nseg)
+        lep_compact_kernel<<<nseg, 256, 0, ctx->stream>>>(static_cast<const SegDesc*>(ctx->d_segs.p), d_offs, static_cast<uint8_t*>(ctx->d_dense.p), nseg);
+    else
+        lep_compact4_kernel<<<nseg, 256, 0, ctx->stream>>>(static_cast<const SegDesc*>(ctx->d_segs.p), d_offs, static_cast<uint8_t*>(ctx->d_dense.p), nseg);
     CK(cudaGetLastError());
     ctx->launches += 1;
     if (total) CK(cudaMemcpyAsync(ctx->h_dense.p, ctx->d_dense.p, total, cudaMemcpyDeviceToHost, ctx->stream));
     CK(cudaStreamSynchronize(ctx->stream));
+    const std::vector<int>& seg_out = ctx->batch.seg_out;          // the caller's order of the segments (plan_batch)
     for (int s = 0; s < nseg; ++s) {
-        out[s].data = static_cast<const uint8_t*>(ctx->h_dense.p) + offs[s];
-        out[s].len = hs[s].status == 0 ? hs[s].len : 0;
-        out[s].status = hs[s].status;
-        out[s].reserved = 0;
-        out[s].ndecisions = (uint64_t)hs[s].ndecisions_lo | ((uint64_t)hs[s].ndecisions_hi << 32);
+        lepb200_stream& o = out[seg_out.empty() ? s : seg_out[s]];
+        o.data = static_cast<const uint8_t*>(ctx->h_dense.p) + offs[s];
+        o.len = hs[s].status == 0 ? hs[s].len : 0;
+        o.status = hs[s].status;
+        o.reserved = 0;
+        o.ndecisions = (uint64_t)hs[s].ndecisions_lo | ((uint64_t)hs[s].ndecisions_hi << 32);
     }
     return LEPB200_OK;
 }
@@ -766,6 +816,10 @@ int lepb200_encode_fetch(lepb200_ctx* ctx, lepb200_stream* out) {
 // bytes are moved by lep_gather_kernel, the LE32 size trailer (vp8_encoder.cc:603-614) is a literal.
 int lepb200_encode_fetch_files(lepb200_ctx* ctx, const lepb200_buffer* headers, lepb200_result* files) {
     if (!ctx || !ctx->launched || !ctx->is_encode || !headers || !files) { if (ctx) ctx->err = "encode_fetch_files without encode_launch"; return LEPB200_ERR_INVALID; }
+    if (ctx->batch.order_ans != (int)ctx->batch.segs.size()) {
+        ctx->err = "encode_fetch_files: rANS-coded segments (container version 3) have no device file writer; fetch them with encode_fetch";
+        return LEPB200_ERR_INVALID;
+    }
     CK(cudaSetDevice(ctx->device));
     const int nseg = (int)ctx->batch.segs.size(), nimg = (int)ctx->batch.images.size();
     CK(ctx->h_segs.reserve(sizeof(SegDesc) * nseg));
@@ -833,7 +887,11 @@ int lepb200_encode_fetch_files(lepb200_ctx* ctx, const lepb200_buffer* headers, 
 }
 
 int lepb200_encode_images(lepb200_ctx* ctx, const lepb200_image* images, int nimages, lepb200_stream* out) {
-    int r = lepb200_encode_upload(ctx, images, nimages);
+    return lepb200_encode_images_coded(ctx, images, nimages, nullptr, out);
+}
+
+int lepb200_encode_images_coded(lepb200_ctx* ctx, const lepb200_image* images, int nimages, const uint8_t* coders, lepb200_stream* out) {
+    int r = lepb200_encode_upload_coded(ctx, images, nimages, coders);
     if (r) return r;
     r = lepb200_encode_launch(ctx);
     if (r) return r;
@@ -845,7 +903,16 @@ int lepb200_encode_images(lepb200_ctx* ctx, const lepb200_image* images, int nim
 // into nfiles files (consecutive, seg_per_file[f] each) for lepb200_encode_fetch_files.
 int lepb200_encode_upload_tokens(lepb200_ctx* ctx, const uint16_t* tokens, const uint32_t* ntok, const uint32_t* caps, int nseg,
                                  const int32_t* seg_per_file, int nfiles) {
+    return lepb200_encode_upload_tokens_coded(ctx, tokens, ntok, caps, nseg, seg_per_file, nfiles, nullptr);
+}
+
+// coders[s]: the coder of segment s.  As in plan_batch, the bool-coded segments come first in the batch's records
+// (BatchPlan::seg_out) and in the launch order; an rANS-coded segment's stream lands in its token slot, not in caps[s].
+int lepb200_encode_upload_tokens_coded(lepb200_ctx* ctx, const uint16_t* tokens, const uint32_t* ntok, const uint32_t* caps, int nseg,
+                                       const int32_t* seg_per_file, int nfiles, const uint8_t* coders) {
     if (!ctx || !tokens || !ntok || !caps || nseg <= 0 || !seg_per_file || nfiles <= 0) return LEPB200_ERR_INVALID;
+    for (int s = 0; coders && s < nseg; ++s)
+        if (coders[s] > LEPB200_CODER_ANS) { ctx->err = "encode_upload_tokens: invalid entropy coder"; return LEPB200_ERR_INVALID; }
     CK(cudaSetDevice(ctx->device));
     ctx->have_batch = ctx->launched = ctx->symbolised = ctx->decode_fetched = false; ctx->is_encode = true; ctx->canary = true;
     BatchPlan& b = ctx->batch;
@@ -874,12 +941,26 @@ int lepb200_encode_upload_tokens(lepb200_ctx* ctx, const uint16_t* tokens, const
         }
     }
     if (s != nseg) { ctx->err = "encode_upload_tokens: seg_per_file does not add up to nseg"; return LEPB200_ERR_INVALID; }
-    b.order.resize(nseg);
-    for (int i = 0; i < nseg; ++i) b.order[i] = i;
-    std::stable_sort(b.order.begin(), b.order.end(), [&](int x, int y) { return ntok[x] > ntok[y]; });
     std::vector<uint16_t> tok((size_t)b.token_total, 0);
     size_t src = 0;
     for (int i = 0; i < nseg; ++i) { memcpy(tok.data() + b.segs[i].tokens, tokens + src, (size_t)ntok[i] * 2); src += ntok[i]; }
+    auto ans = [&](int x) { return coders && coders[x] == LEPB200_CODER_ANS; };
+    b.seg_out.clear();
+    if (coders && std::any_of(coders, coders + nseg, [](uint8_t c) { return c == LEPB200_CODER_ANS; })) {
+        b.seg_out.resize(nseg);
+        for (int i = 0; i < nseg; ++i) b.seg_out[i] = i;
+        std::stable_partition(b.seg_out.begin(), b.seg_out.end(), [&](int x) { return !ans(x); });
+        std::vector<SegDesc> segs(nseg);
+        for (int d = 0; d < nseg; ++d) segs[d] = b.segs[b.seg_out[d]];
+        b.segs.swap(segs);
+    }
+    auto caller = [&](int d) { return b.seg_out.empty() ? d : b.seg_out[d]; };
+    b.order.resize(nseg);
+    for (int i = 0; i < nseg; ++i) b.order[i] = i;
+    std::stable_sort(b.order.begin(), b.order.end(), [&](int x, int y) {
+        return ans(caller(x)) != ans(caller(y)) ? ans(caller(y)) : ntok[caller(x)] > ntok[caller(y)]; });
+    b.order_ans = nseg;
+    while (b.order_ans > 0 && ans(caller(b.order[b.order_ans - 1]))) --b.order_ans;
     CK(ctx->d_streams.reserve(b.stream_total + 256));
     CK(ctx->d_tokens.reserve((size_t)b.token_total * 2 + 256));
     CK(ctx->d_images.reserve(sizeof(ImageDesc) * nfiles));
@@ -917,7 +998,7 @@ int lepb200_encode_token_canaries(lepb200_ctx* ctx, uint8_t* moved, uint64_t* ch
     for (int s = 0; s < nseg; ++s) {
         const size_t slot = (size_t)(b.segs[s].stream - base), end = slot + align_up((size_t)b.segs[s].cap + CANARY_BYTES, 256);
         for (size_t k = slot + b.segs[s].cap; k < end; ++k) bad += arena[k] != CANARY_BYTE;
-        moved[s] = hs[s].stream < base || hs[s].stream >= base + b.stream_total;
+        moved[b.seg_out.empty() ? s : b.seg_out[s]] = hs[s].stream < base || hs[s].stream >= base + b.stream_total;
     }
     for (uint8_t c : tail) bad += c != CANARY_BYTE;
     *changed = bad;

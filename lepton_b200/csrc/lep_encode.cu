@@ -60,6 +60,21 @@ struct EncWarpSmem {
 // (the CTA's shared memory is declared as separate arrays inside the kernel: members of one struct reached through a
 // reference made the compiler build generic addresses -- shared-window base from a special register -- at several uses)
 
+// ---- the coder's model ------------------------------------------------------------------------------------
+// Kernel A codes the same decisions for both entropy coders; only the branch model differs: the bool coder's
+// (record_obs_and_update, two absorbing states) or the rANS coder's (adv_record_obs_and_update, no absorbing state, see
+// lep_common.cuh).  Both leave tokens of the same format, probability | bit << 8.
+struct EncBool {
+    static constexpr bool kAbsorbing = true;          // the model has states a branch cannot leave (flush_queue)
+    __device__ static __forceinline__ uint32_t prob(uint32_t w, const uint32_t* __restrict__ s_rcp) { return branch_prob(w, s_rcp); }
+    __device__ static __forceinline__ uint32_t update(uint32_t w, uint32_t bit) { return branch_update(w, bit); }
+};
+struct EncAns {
+    static constexpr bool kAbsorbing = false;
+    __device__ static __forceinline__ uint32_t prob(uint32_t w, const uint32_t* __restrict__ s_rcp) { return branch_prob_ans(w, s_rcp); }
+    __device__ static __forceinline__ uint32_t update(uint32_t w, uint32_t bit) { return branch_update_ans(w, bit); }
+};
+
 // ---- queue flush: expansion of the items + batched model update ---------------------------------------
 __device__ __forceinline__ uint32_t expand_item(const uint4 d, int pos) {      // pos: position relative to the item's block
     if (d.x >> 31) return d.y;
@@ -76,7 +91,7 @@ __device__ __forceinline__ uint32_t expand_item(const uint4 d, int pos) {      /
 }
 
 // n queued positions; the items of block B (ids >= N_ITEMS) are positioned relative to base_b
-__device__ __forceinline__ void flush_queue(EncWarpSmem& ws, int n, int base_b, uint16_t* __restrict__ model,
+template <class Model> __device__ __forceinline__ void flush_queue(EncWarpSmem& ws, int n, int base_b, uint16_t* __restrict__ model,
                                             const uint32_t* __restrict__ s_rcp, uint16_t* __restrict__ tokens, uint32_t& ntok,
                                             uint32_t tok_cap, int lane) {
     const uint32_t lt_mask = (1u << lane) - 1, le_mask = lt_mask | (1u << lane);
@@ -111,13 +126,17 @@ __device__ __forceinline__ void flush_queue(EncWarpSmem& ws, int n, int base_b, 
         uint32_t w = active ? (uint32_t)model[addr] : 0u;
         // Resolve same-branch conflicts in queue order.  While no count of the group can saturate inside this batch
         // (the common case) record_obs_and_update is a plain increment, so the state a lane sees is the loaded word
-        // plus the number of zeros / ones its predecessors on the same branch observed: closed form, no rounds.
+        // plus the number of zeros / ones its predecessors on the same branch observed: closed form, no rounds.  So does
+        // the rANS model's update below 255 (its low byte never reaches 0xff).
         const uint32_t ones = __ballot_sync(FULL, bit != 0);
         const uint32_t n1_all = __popc(peers & ones), n0_all = __popc(peers & ~ones);
         const bool plain = !active || ((w & 0xff) + n0_all <= 254u && (w >> 8) + n1_all <= 254u);   // low byte 0xff (special state) never passes
-        // the two absorbing states: (255,1) seeing only zeros and the "neverseen" (1,255) seeing only ones do not move
-        // (branch.hh:87-99); branches that always code the same bit sit there for good
-        const bool stuck = (w == 0x00feu && n1_all == 0) || ((w & 0xff) == 0xffu && n0_all == 0);
+        // the two absorbing states of the bool model: (255,1) seeing only zeros and the "neverseen" (1,255) seeing only
+        // ones do not move (branch.hh:87-99); branches that always code the same bit sit there for good.  The rANS model
+        // restarts such a count at 129 and has none.  (Written as a reset, not as `kAbsorbing && ...`: that form changes
+        // the bool kernel's SASS.)
+        bool stuck = (w == 0x00feu && n1_all == 0) || ((w & 0xff) == 0xffu && n0_all == 0);
+        if (!Model::kAbsorbing) stuck = false;
         uint32_t neww;                                            // state after this lane's own observation
         if (__all_sync(FULL, plain || stuck)) {
             if (!stuck) w += __popc(earlier & ~ones) + (__popc(earlier & ones) << 8);
@@ -129,13 +148,13 @@ __device__ __forceinline__ void flush_queue(EncWarpSmem& ws, int n, int base_b, 
             const int pred = earlier ? 31 - __clz(earlier) : lane;     // previous decision on the same branch
             const int maxrank = __reduce_max_sync(FULL, rank);
             for (int r = 1; r <= maxrank; ++r) {
-                const uint32_t after = branch_update(w, bit);
+                const uint32_t after = Model::update(w, bit);
                 const uint32_t from_pred = __shfl_sync(FULL, after, pred);
                 if (rank == r) w = from_pred;
             }
-            neww = branch_update(w, bit);
+            neww = Model::update(w, bit);
         }
-        const uint32_t pb = branch_prob(w, s_rcp) | (bit << 8);
+        const uint32_t pb = Model::prob(w, s_rcp) | (bit << 8);
         if (active && (peers >> lane) == 1u) model[addr] = (uint16_t)neww;                    // last decision of its branch
         if (active && ntok + i < tok_cap) LEP_ST_STREAM(tokens, ntok + i, (uint16_t)pb);                    // coalesced 2-byte stores
         __syncwarp();                                                                         // order this batch's model stores before the next batch's loads
@@ -244,6 +263,9 @@ __device__ __forceinline__ int lak_pred_at(const EncWarpSmem& ws, int cur_off, i
 #ifndef LEPB200_ENC_MINBLOCKS
 #define LEPB200_ENC_MINBLOCKS 6
 #endif
+// Model: the coder's branch model, EncBool (container versions 1, 2 and 4) or EncAns (version 3).  order[0 .. nseg) are
+// the launch's segments, all of the one coder.
+template <class Model = EncBool>
 __global__ void __launch_bounds__(ENC_WARPS_PER_CTA * 32, LEPB200_ENC_MINBLOCKS)
 lep_encode_kernel(const ImageDesc* __restrict__ images, SegDesc* __restrict__ segs, int nseg, const int* __restrict__ order,
                   int* __restrict__ work_counter, uint16_t* __restrict__ model_pool, uint8_t* __restrict__ row_pool,
@@ -560,7 +582,7 @@ lep_encode_kernel(const ImageDesc* __restrict__ images, SegDesc* __restrict__ se
                 // ---------------- code the queued decisions
                 status = __reduce_max_sync(FULL, status);
                 if (status != ST_OK) break;
-                flush_queue(ws, qnA + qnB, base_b, model, s_rcp, tokens, ntok, tok_cap, lane);
+                flush_queue<Model>(ws, qnA + qnB, base_b, model, s_rcp, tokens, ntok, tok_cap, lane);
                 ndec += (unsigned long long)(qnA + qnB);
                 if (!more) break;
                 aleft = abvB; left = curB;
@@ -580,6 +602,7 @@ lep_encode_kernel(const ImageDesc* __restrict__ images, SegDesc* __restrict__ se
         __syncwarp();
     }
 }
+
 
 // ---- kernel B: the range coder, one thread per segment ------------------------------------------------
 // vpx_start_encode / vpx_write / vpx_stop_encode (src/vp8/encoder/boolwriter.cc:17-35, boolwriter.hh:48-118)
@@ -1044,6 +1067,157 @@ lep_rangenorm_kernel(SegDesc* __restrict__ segs, int nseg, const int* __restrict
         sd.stream = (unsigned long long)(uintptr_t)buf;               // where lep_compact_kernel and lep_gather_kernel find it
         if (len >= cap) sd.status = ST_OUT_OVERFLOW;
     }
+}
+
+// ---- the rANS pass: a segment's tokens -> the reference's rANS stream (container version 3) ----------------------
+// ANSBoolWriter::finish (ans_bool_writer.hh:66-107, rans64.hh:60-100) over kernel A's tokens, one THREAD per segment.  The
+// decisions form pairs (2k, 2k + 1), an odd count completed by a pad (p = 1, bit 1), and 4 pairs of (p = 128, bit 0) follow
+// the last pair.  The pairs are coded last to first, the odd decision (state A) before the even one (state B): the two
+// states are two independent chains, which the thread runs side by side.  A state x in [2^31, 2^63) that is at or above
+// 2^55 * freq first emits its low 32 bits; then x = (x / freq) * 256 + x % freq + start, where [start, start + freq) is the
+// decision's share of [0, 256): [0, p) for bit 0, [p, 256) for bit 1.  The stream is the two final states (B then A, low
+// word first), the emitted words last to first, and the 4 bytes 00 80 00 80.
+//
+// Division by freq in [1, 256] without a 64-bit divide (ans_divide): with l = ceil(log2 freq) and m = ceil(2^(63+l) / freq)
+// (< 2^64: freq > 2^(l-1) or m = 2^63), q = mulhi64(2x, m) >> l = floor(x m / 2^(63+l)).  Exact for every x < 2^63
+// (Granlund & Montgomery, PLDI 1994, thm 4.2): m freq = 2^(63+l) + e with 0 <= e < freq <= 2^l, so
+// x m / 2^(63+l) = x / freq + x e / (freq 2^(63+l)), and the second term is < 2^63 2^l / (freq 2^(63+l)) = 1 / freq;
+// x / freq = q + r / freq with r <= freq - 1, so the sum stays below q + 1.  (2x < 2^64 because x < 2^63.)  The
+// remainder is x - q freq, taken in 32 bits.  tests/test_emu_ans_encode.py checks every freq at x = k freq - 1, k freq,
+// 2^55 freq +- 1 and 2^63 - 1.
+//
+// Output bound: a state stays >= 2^31 and a decision multiplies x + 1 by at most 256 (x' <= 256 floor(x / freq) + 255),
+// an emission divides it by 2^32 up to a factor 1 + 2^-23 (x >= 2^55 there).  So after m decisions on a state,
+// 31 + 32 e <= log2(x + 1) + 32 e <= 31 + m (8 + 1.8e-7): e <= (m + (m >> 25)) / 4 words.  With M <= ntok + 9 decisions
+// in all the stream is at most 20 + M + (M >> 25) bytes: ans_stream_bound (ntok + 40 up to 2^25 tokens).  The words are
+// written in place, backward from the end of the segment's token slot of C = 2 tok_cap bytes (the reference writes over
+// its symbol buffer the same way, ans_bool_writer.hh:90-97).  Once the decisions from token j on are coded, at most
+// W = 4 + M_j + (M_j >> 25) <= ans_stream_bound(ntok) - j - 16 bytes are written (M_j <= ntok - j + 9), so the lowest byte
+// written, C - W, lies above the 2 j bytes of the tokens still to be read as long as C >= ntok + ans_stream_bound(ntok)
+// (ans_slot_fits; token_slot gives C >= 2 ntok + 128, enough below 3 * 10^9 tokens).  So an rANS stream needs no stream
+// slot, no overflow arena and no second run; SegDesc::stream / len point at it in the token arena.
+__host__ __device__ constexpr unsigned long long ans_stream_bound(unsigned long long ntok) {
+    return ntok + 29 + ((ntok + 9) >> 25);
+}
+__host__ __device__ constexpr bool ans_slot_fits(unsigned long long ntok, unsigned long long tok_cap) {
+    return ntok <= tok_cap && 2 * tok_cap >= ntok + ans_stream_bound(ntok);
+}
+// l = ceil(log2 f) and m = ceil(2^(63+l) / f) for f in [1, 256] (long division in 32-bit limbs: set-up only, not the chain)
+__host__ __device__ constexpr int ans_recip_shift(uint32_t f) {
+    int l = 0;
+    while ((1u << l) < f) ++l;
+    return l;
+}
+__host__ __device__ constexpr unsigned long long ans_recip(uint32_t f) {
+    const int l = ans_recip_shift(f);
+    if ((f & (f - 1)) == 0) return 1ull << 63;                             // f = 2^l
+    // 2^(63+l) = a 2^64 with a = 2^(l-1) < f: quotient < 2^64
+    const unsigned long long a = 1ull << (l - 1);
+    const unsigned long long q1 = (a << 32) / f, r1 = (a << 32) % f;
+    const unsigned long long q0 = (r1 << 32) / f, r0 = (r1 << 32) % f;
+    return (q1 << 32) + q0 + (r0 != 0 ? 1 : 0);
+}
+#ifndef LEPB200_EMU
+__device__ __forceinline__ unsigned long long ans_mulhi64(unsigned long long a, unsigned long long b) { return __umul64hi(a, b); }
+#else
+inline unsigned long long ans_mulhi64(unsigned long long a, unsigned long long b) { return (unsigned long long)(((unsigned __int128)a * b) >> 64); }
+#endif
+// floor(x / f) and x % f for x < 2^63, f in [1, 256]: m = ans_recip(f), l = ans_recip_shift(f)
+__device__ __forceinline__ unsigned long long ans_divide(unsigned long long x, uint32_t f, unsigned long long m, int l, uint32_t& r) {
+    const unsigned long long q = ans_mulhi64(x << 1, m) >> l;
+    r = (uint32_t)x - (uint32_t)q * f;
+    return q;
+}
+
+constexpr int ANS_THREADS = 32;
+constexpr int ANS_DEPTH = 8;                               // 16-byte token loads in flight per thread (a register ring)
+
+struct AnsPut { unsigned long long m; uint32_t f, start; int l; };
+// the decision's share of [0, 256) and its reciprocal: off the states' chains (they depend on the token only)
+__device__ __forceinline__ AnsPut ans_token(uint32_t tok, const unsigned long long* __restrict__ s_m, uint32_t& bad) {
+    const uint32_t p = tok & 0xffu, bit = (tok >> 8) & 1u;
+    AnsPut d;
+    // the reference's writer asserts on a probability 0 (kernel A never produces one; the token test entry can pass one):
+    // such a decision is coded as freq 256 (no bit at all) so that every decision keeps freq in [1, 256] -- the bound the
+    // in-place writes rely on -- and the segment ends with status 1, its stream discarded
+    d.f = ((bit ? 256u - p : p) - 1u & 255u) + 1u;         // p = 0, bit 0 gives 0 -> 256
+    d.start = bit ? p : 0u;
+    bad |= p == 0u ? 1u : 0u;
+    d.m = s_m[d.f - 1u];
+    d.l = 32 - __clz(d.f - 1u);                            // ceil(log2 f); f = 1: 0
+    return d;
+}
+// Rans64EncPut at scale 8: one decision on state x; an emitted word goes to *--wp
+__device__ __forceinline__ void ans_put(unsigned long long& x, const AnsPut& d, uint32_t*& wp) {
+    if ((uint32_t)(x >> 55) >= d.f) {                      // x >= 2^55 f
+#ifndef LEPB200_EMU
+        asm volatile("st.global.u32 [%0], %1;" ::"l"(wp - 1), "r"((uint32_t)x) : "memory");
+#else
+        wp[-1] = (uint32_t)x;
+#endif
+        --wp;
+        x >>= 32;
+    }
+    uint32_t r;
+    const unsigned long long q = ans_divide(x, d.f, d.m, d.l, r);
+    x = (q << 8) + r + d.start;
+}
+
+__global__ void __launch_bounds__(ANS_THREADS)
+lep_anspass_kernel(SegDesc* __restrict__ segs, int nseg, const int* __restrict__ order, uint16_t* token_base) {
+    __shared__ unsigned long long s_m[256];
+    for (int i = threadIdx.x; i < 256; i += ANS_THREADS) s_m[i] = ans_recip((uint32_t)i + 1u);
+    __syncthreads();
+    const int t = blockIdx.x * ANS_THREADS + threadIdx.x;
+    if (t >= nseg) return;
+    SegDesc& sd = segs[order[t]];
+    if (sd.status != ST_OK) return;                        // kernel A's status (100: token overflow) stays
+    const uint32_t ntok = sd.ntok;
+    if (!ans_slot_fits(ntok, sd.tok_cap)) { sd.status = ST_OUT_OVERFLOW; sd.len = 0; return; }
+    // the token slot is read and written by this thread only: plain loads (no read-only path), written behind the reads
+    uint16_t* tok = token_base + sd.tokens;
+    uint32_t* const end = reinterpret_cast<uint32_t*>(tok + sd.tok_cap);
+    uint32_t* wp = end;
+    *--wp = 0x80008000u;                                   // 00 80 00 80: the unused pair of the reference's symbol buffer
+    unsigned long long a = 1ull << 31, b = 1ull << 31;     // RANS64_L
+    uint32_t bad = 0;
+    const AnsPut mid = ans_token(128u, s_m, bad);
+#pragma unroll 1
+    for (int i = 0; i < 4; ++i) { ans_put(a, mid, wp); ans_put(b, mid, wp); }   // the 4 trailing (128, 0) pairs
+    // decision j goes to state A when j is odd (the second of its pair), to B when it is even; descending j is the coding order
+    if (ntok & 1u) ans_put(a, ans_token(0x101u, s_m, bad), wp);                  // pad of an odd count: (p = 1, bit 1)
+    const uint32_t nfull = ntok / 8;
+#pragma unroll 1
+    for (uint32_t j = ntok; j-- > nfull * 8;) {
+        const AnsPut d = ans_token(tok[j], s_m, bad);
+        if (j & 1u) ans_put(a, d, wp); else ans_put(b, d, wp);
+    }
+    // whole 16-byte groups, last to first, ANS_DEPTH loads ahead
+    const uint4* tok4 = reinterpret_cast<const uint4*>(tok);
+    uint4 q[ANS_DEPTH];
+#pragma unroll
+    for (int k = 0; k < ANS_DEPTH; ++k) q[k] = (uint32_t)k < nfull ? tok4[nfull - 1 - k] : make_uint4(0, 0, 0, 0);
+    for (uint32_t base = 0; base < nfull; base += ANS_DEPTH) {
+#pragma unroll
+        for (int k = 0; k < ANS_DEPTH; ++k) {
+            const uint32_t i = base + (uint32_t)k;           // group nfull - 1 - i
+            if (i < nfull) {
+                const uint4 cur = q[k];
+                q[k] = i + ANS_DEPTH < nfull ? tok4[nfull - 1 - i - ANS_DEPTH] : make_uint4(0, 0, 0, 0);
+                // tokens 7 (A), 6 (B), 5 (A), ... 0 (B) of the group
+                ans_put(a, ans_token(cur.w >> 16, s_m, bad), wp); ans_put(b, ans_token(cur.w & 0xffffu, s_m, bad), wp);
+                ans_put(a, ans_token(cur.z >> 16, s_m, bad), wp); ans_put(b, ans_token(cur.z & 0xffffu, s_m, bad), wp);
+                ans_put(a, ans_token(cur.y >> 16, s_m, bad), wp); ans_put(b, ans_token(cur.y & 0xffffu, s_m, bad), wp);
+                ans_put(a, ans_token(cur.x >> 16, s_m, bad), wp); ans_put(b, ans_token(cur.x & 0xffffu, s_m, bad), wp);
+            }
+        }
+    }
+    // the head: B's state, then A's, low word first
+    *--wp = (uint32_t)(a >> 32); *--wp = (uint32_t)a;
+    *--wp = (uint32_t)(b >> 32); *--wp = (uint32_t)b;
+    if (bad) { sd.status = ST_ASSERT; sd.len = 0; return; }
+    sd.stream = (unsigned long long)(uintptr_t)wp;          // where the fetch finds it (4-byte aligned, in the token arena)
+    sd.len = (uint32_t)((end - wp) * 4);
 }
 
 // ---- pre-pass: upper bound of the number of tokens each segment will produce -------------------------------

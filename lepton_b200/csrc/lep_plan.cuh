@@ -91,8 +91,12 @@ inline uint32_t token_slot(unsigned long long bound) {
 struct BatchPlan {
     std::vector<ImageDesc> images;        // plane[c]: offset in the plane arena
     std::vector<SegDesc> segs;            // stream: offset in the stream arena; tokens: offset in the token arena (tokens_known)
-    std::vector<int> order;               // bool-coded segments, then rANS-coded ones (decode), each part largest first
-    int order_ans = 0;                    // decode: order[order_ans ..] are the rANS-coded segments (CODER_ANS)
+    std::vector<int> order;               // bool-coded segments, then rANS-coded ones, each part largest first
+    int order_ans = 0;                    // order[order_ans ..] are the rANS-coded segments (CODER_ANS)
+    // encode batches with rANS-coded segments: segs holds the bool-coded segments first, then the rANS-coded ones (each in
+    // image order), so that the range coder's launches, which take segments by index, take only the first order_ans;
+    // seg_out[d] = the caller's index (image after image) of segs[d].  Empty: segs is in the caller's order.
+    std::vector<int> seg_out;
     std::vector<size_t> seg_blocks;       // blocks each segment codes
     std::vector<size_t> plane_bytes;      // per image * 3 + component
     size_t plane_total = 0, stream_total = 0, row_stride = 0;
@@ -102,13 +106,13 @@ struct BatchPlan {
 
 // Job tables of an encode (in = nullptr) or decode batch (in = one stream per segment): ImageDesc / SegDesc, the plane arena
 // (256-byte aligned planes), the stream arena, the row stride of the kernels' row buffers and the launch order.  coders
-// (decode, optional): the entropy coder of each image's streams (LEPB200_CODER_BOOL / LEPB200_CODER_ANS); nullptr = all bool.
+// (optional): the entropy coder of each image's streams (LEPB200_CODER_BOOL / LEPB200_CODER_ANS); nullptr = all bool.
 // Returns nullptr, or what is wrong with the batch.
 inline const char* plan_batch(BatchPlan& b, const lepb200_image* images, int nimages, bool encode, const lepb200_stream* in,
                               const uint8_t* coders = nullptr) {
     if (nimages <= 0 || !images) return "empty batch";
     b.images.assign(nimages, ImageDesc());
-    b.segs.clear(); b.seg_blocks.clear(); b.plane_bytes.assign((size_t)nimages * 3, 0);
+    b.segs.clear(); b.seg_blocks.clear(); b.seg_out.clear(); b.plane_bytes.assign((size_t)nimages * 3, 0);
     b.plane_total = b.stream_total = b.row_stride = 0;
     b.token_total = 0;
     b.tokens_known = encode;
@@ -116,7 +120,7 @@ inline const char* plan_batch(BatchPlan& b, const lepb200_image* images, int nim
     for (int i = 0; i < nimages; ++i) {
         const lepb200_image& im = images[i];
         if (const char* e = validate_image(im)) return e;
-        if (coders && (encode || coders[i] > LEPB200_CODER_ANS)) return "invalid entropy coder";
+        if (coders && coders[i] > LEPB200_CODER_ANS) return "invalid entropy coder";
         ImageDesc& d = b.images[i];
         memset(&d, 0, sizeof(d));
         d.ncmp = im.ncmp; d.mcuv = im.mcuv;
@@ -150,7 +154,8 @@ inline const char* plan_batch(BatchPlan& b, const lepb200_image* images, int nim
                 // such a stream moves to the overflow arena, sized from the exact length (parallel range coder, see
                 // lep_digit_offsets_kernel) or from a proven bound when the serial coder codes the segment again
                 // (plan_serial_rerun).  No stream is ever cut short.
-                size_t cap = align_up(nb * 64 + 4096, 256);
+                // An rANS segment's stream is written into its token slot (lep_anspass_kernel): no stream slot.
+                size_t cap = d.coder == CODER_ANS ? 0 : align_up(nb * 64 + 4096, 256);
                 sd.stream = b.stream_total; sd.cap = (uint32_t)cap;
                 b.stream_total += cap;
                 sd.tokens = 0; sd.tok_cap = 0;                    // assigned on the device by the counting pre-pass ...
@@ -168,12 +173,22 @@ inline const char* plan_batch(BatchPlan& b, const lepb200_image* images, int nim
             b.segs.push_back(sd);
         }
     }
-    // largest segments first (longest-processing-time-first on the persistent warps); a decode kernel launch takes the
-    // segments of one coder, so those of the rANS coder follow all the others
     const int nseg = (int)b.segs.size();
+    auto coder = [&](int x) { return b.images[b.segs[x].image].coder; };
+    if (encode && std::any_of(b.images.begin(), b.images.end(), [](const ImageDesc& d) { return d.coder == CODER_ANS; })) {
+        b.seg_out.resize(nseg);
+        for (int i = 0; i < nseg; ++i) b.seg_out[i] = i;
+        std::stable_partition(b.seg_out.begin(), b.seg_out.end(), [&](int x) { return coder(x) != CODER_ANS; });
+        std::vector<SegDesc> segs(nseg);
+        std::vector<size_t> blocks(nseg);
+        for (int d = 0; d < nseg; ++d) { segs[d] = b.segs[b.seg_out[d]]; blocks[d] = b.seg_blocks[b.seg_out[d]]; }
+        b.segs.swap(segs);
+        b.seg_blocks.swap(blocks);
+    }
+    // largest segments first (longest-processing-time-first on the persistent warps); a kernel launch takes the segments
+    // of one coder, so those of the rANS coder follow all the others
     b.order.resize(nseg);
     for (int i = 0; i < nseg; ++i) b.order[i] = i;
-    auto coder = [&](int x) { return b.images[b.segs[x].image].coder; };
     std::stable_sort(b.order.begin(), b.order.end(), [&](int x, int y) {
         return coder(x) != coder(y) ? coder(x) < coder(y) : b.seg_blocks[x] > b.seg_blocks[y]; });
     b.order_ans = nseg;
